@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native MegReader recognition hot path.
+"""bench.py — headline benchmark of the H100-native MegReader recognition hot path.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
 
@@ -14,7 +14,7 @@ Prints ONE JSON line (rank 0).  Extra objects on that line:
   ctc2d        second half of BASELINE.json's metric: 2D-CTC fwd+bwd GB/s at the cfg-3 shape, saturating batch
   cpu_baseline the oracle port of the same step timed on this box's host cores (bounded sample)
 --impl reference runs only the CPU arm (oracle port = restatement of the reference's own CPU path; the python
-reference itself cannot travel to the GPU box) and prints the same line shape with "impl": "reference".
+reference itself is not part of this repository) and prints the same line shape with "impl": "reference".
 """
 import argparse
 import json
@@ -43,7 +43,9 @@ def peaks():
         d = json.load(open(p))
         return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d["bf16_tflops"]),
                 "bf16_tflops_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0,
+            "bf16_tflops_sustained": 989.0,      # no sustained figure without a measurement: the data-sheet peak again
+            "source": "H100 SXM data sheet (700 W); sustained = peak, not measured"}
 
 
 # ---------------------------------------------------------------------------------------------- clocks sampler
@@ -101,7 +103,7 @@ def headline_config(batch, world):
                         "bf16 autocast compute, Adam lr 1e-3", "batch_per_gpu": batch,
             "global_batch": batch * world, "T": T_COLS, "classes": 38, "parallelism": "dp%d" % world,
             "l2": "3 rotating input batches (50 MB each) + 33 MB params/grads/Adam state per step exceed reuse; "
-                  "activations (>1 GB/step) far exceed the 126 MB L2"}
+                  "activations (>1 GB/step) far exceed the 50 MB L2"}
 
 
 # ---------------------------------------------------------------------------------------------- our arm
@@ -121,6 +123,24 @@ def build_model(device):
         def forward(self, images, targets, lengths):
             return self.decoder(self.backbone(images), targets=targets, lengths=lengths, train=True)
     return Net().to(device).train()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(path, arrays):
+    """Write each array as <path>/<name>.npy (float32; float64 stays float64).  Together they stay under DUMP_LIMIT_BYTES:
+    a larger array is cut down to a fixed, seeded sample of its elements, the same from run to run."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    budget = DUMP_LIMIT_BYTES // max(1, len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        a = a.astype(np.float64 if a.dtype == np.float64 else np.float32).reshape(-1)
+        keep = budget // a.itemsize
+        if a.size > keep:
+            a = a[np.sort(np.random.RandomState(1234).choice(a.size, keep, replace=False))]
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 def run_ours(args):
@@ -235,6 +255,12 @@ def run_ours(args):
     ms = e0.elapsed_time(e1)
     clocks = sampler.stop() if sampler else None
     final_loss = float(loss.mean().item())
+    if args.dump_outputs and rank == 0:
+        # what the last timed step returned to its caller: the per-line losses and the weights after its Adam update
+        dump_outputs(args.dump_outputs, {
+            "loss": loss.detach().reshape(-1),
+            "params": torch.cat([p.detach().reshape(-1).float() for p in params]),
+        })
 
     # ---- end-to-end arm: host pinned inputs, prefetch on a copy stream, loss read back every step
     copy_stream = torch.cuda.Stream()
@@ -312,9 +338,9 @@ def run_ours(args):
                 out["cpu_baselines_other"] = cpu_side_baselines()
             except Exception as e:
                 out["cpu_baselines_other"] = {"error": str(e)[:200]}
-        out["stages"] = {"conv": "megreader_b200 tcgen05 implicit-GEMM kernels (fprop, dgrad, wgrad); conv0 (Cin=3): im2col kernel + cuBLAS",
+        out["stages"] = {"conv": "megreader_b200 wgmma implicit-GEMM kernels (fprop, dgrad, wgrad); conv0 (Cin=3): im2col kernel + cuBLAS",
                          "bias+ReLU+MaxPool, BatchNorm": "megreader_b200 CUDA (fused NHWC kernels)",
-                         "BiLSTM+Linear": "recurrence: megreader_b200 persistent tcgen05 kernels (one launch per layer and pass, mode '%s'); "
+                         "BiLSTM+Linear": "recurrence: megreader_b200 persistent wgmma kernels (one launch per layer and pass, mode '%s'); "
                                           "input projections / Linear / weight-gradient GEMMs: cuBLAS" % crnn_engine.LSTM_MODE,
                          "conv weight gradients": "side stream, overlapped with the backward chain" if crnn_engine.WGRAD_SIDE_STREAM else "main stream",
                          "log_softmax+CTC": "megreader_b200 CUDA", "Adam": "library (torch fused, capturable)",
@@ -394,7 +420,7 @@ def bench_ctc2d(dev, iters=10):
                    "frac_of_hbm_peak": N * pair_bytes / (tf + tb) / 1e9 / pk["hbm_gbs"], "peak_source": pk["source"]}
             roof = {"kernel": "ctc2d_dp4_kernel<FAC> (2D-CTC training forward: Q, interleaved alpha/beta sweeps, factors)",
                     "bound": "hbm", "achieved": N * fwd_bytes / tf / 1e9, "peak": pk["hbm_gbs"], "unit": "GB/s",
-                    "frac": N * fwd_bytes / tf / 1e9 / pk["hbm_gbs"], "traffic": _measured("ctc2d_dp4", "dram_bytes_per_launch"),
+                    "frac": N * fwd_bytes / tf / 1e9 / pk["hbm_gbs"],
                     "peak_source": pk["source"], "alg_bytes_per_launch": N * fwd_bytes,
                     "note": "2D-CTC training forward (BASELINE.json metric, second half)"}
             # head epilogue in front of the loss (decoders/ctc_decoder2d.py:37-45): logits -> log_probs, and the fused backward
@@ -427,18 +453,8 @@ def bench_ctc2d(dev, iters=10):
     return ctc, roof
 
 
-def _measured(kernel, key):
-    """A number taken from the committed ncu summary of the current revision (profiles/measured_r2.json, written from the
-    `ncu --set full` captures listed in profiles/); None when no capture of that kernel is committed."""
-    try:
-        d = json.load(open(os.path.join(ROOT, "profiles", "measured_r2.json")))
-        return d[kernel][key]
-    except Exception:
-        return None
-
-
 def bench_dcn(dev, iters=10):
-    """DCNv2 forward at SURVEY.md section 8d's shapes (B = 8): fused tcgen05 implicit GEMM (csrc/dcn_tcgen05.cu), timed through the
+    """DCNv2 forward at SURVEY.md section 8d's shapes (B = 8): fused wgmma implicit GEMM (csrc/dcn_tcgen05.cu), timed through the
     autograd surface (NHWC copy + weight pack + the GEMM).  Roofline: tensor pipe, 2*C*9*Cout*Ho*Wo flops per sample."""
     from megreader_b200 import dcn
     pk = peaks()
@@ -482,11 +498,7 @@ def bench_dcn(dev, iters=10):
                                         "bwd_frac_of_tensor_peak": 2 * flops / bsec / 1e12 / pk["bf16_tflops"]}
     return {"kernel": "dcn_fwd_tcgen05_kernel (bilinear gather = A-operand producer, bf16 hi/lo split: 3 MMAs per K block); backward = "
                       "dcn_wgrad_tcgen05_kernel + dcn_dgrad_tcgen05_kernel (no column matrices in HBM)",
-            "bound": "tensor", "unit": "TFLOP/s", "peak": pk["bf16_tflops"], "peak_source": pk["source"], "B": 8, "shapes": out,
-            "traffic_bwd_C128@64x64": {"dcn_dgrad_tcgen05_kernel": _measured("dcn_dgrad_c128", "dram_bytes_per_launch"),
-                                       "dcn_wgrad_tcgen05_kernel": _measured("dcn_wgrad_c128", "dram_bytes_per_launch")},
-            "round1_fwd_us": {"C128@64x64": 319.2, "C256@32x32": 264.5, "C512@16x16": 215.3},
-            "round1_fwd_bwd_us": {"C128@64x64": 1611.0, "C256@32x32": 1115.3, "C512@16x16": 944.9}}
+            "bound": "tensor", "unit": "TFLOP/s", "peak": pk["bf16_tflops"], "peak_source": pk["source"], "B": 8, "shapes": out}
 
 
 def bench_input_step(dev, n=512, reps=5):
@@ -562,10 +574,9 @@ def bench_conv_roofline(dev, iters=10):
     sec = a.elapsed_time(b) / iters * 1e-3
     flops = 2.0 * N * H * W * Cout * k * k * C
     pk = peaks()
-    return {"kernel": "conv_fprop_tcgen05_kernel<256,2,1,1> (implicit-GEMM 3x3 conv via 4-D TMA, conv5 shape, bf16 in / fp32 acc)",
+    return {"kernel": "conv_fprop_tcgen05_kernel<128,3,1> (wgmma implicit-GEMM 3x3 conv via 4-D TMA, conv5 shape, bf16 in / fp32 acc)",
             "bound": "tensor", "achieved": flops / sec / 1e12, "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
             "frac": flops / sec / 1e12 / pk["bf16_tflops"],
-            "traffic": _measured("conv_fprop_conv5", "dram_bytes_per_launch"),   # ncu --set full of this revision, or None
             "traffic_algorithmic": 2.0 * N * H * W * C + 2.0 * N * H * W * Cout + 2.0 * Cout * k * k * C,
             "peak_source": pk["source"],
             "alg_flops_per_launch": flops, "us_per_launch": sec * 1e6}
@@ -592,7 +603,7 @@ def usable_cores():
 
 def cpu_arm(steps, warmup, sample_n, budget_s=25.0):
     """The reference's own CPU path for this workload, restated by oracle/crnn_port.py (validated bit-for-bit against
-    the unmodified reference modules in the build container): fp32, all host cores, same model/optimizer."""
+    the unmodified reference modules by tests/test_oracle_crnn.py): fp32, all host cores, same model/optimizer."""
     from oracle import crnn_port
     from tests.weights import fill_state_dict
     cores = usable_cores()
@@ -735,6 +746,8 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (losses, updated weights) as DIR/<name>.npy")
     ap.add_argument("--config", type=int, default=2, choices=[2, 3, 4, 5],
                     help="BASELINE.json configuration: 2 = CRNN + 1D CTC (headline, default); 3 = ResNet50-PPM + 2D CTC; "
                          "4 = FPN50 + attention decoder; 5 = deformable ResNet50 + FPN + EAST (bench_trunks.py)")
@@ -743,6 +756,8 @@ def main():
                     help="reference semantics (data/data_loader.py:40-43): global batch 512 split over the ranks (strong scaling) "
                          "instead of 512 per GPU")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.config != 2):
+        raise SystemExit("--dump-outputs is implemented for the headline configuration only (--impl ours --config 2)")
     if args.impl == "reference":
         run_reference(args)
     elif args.config != 2:

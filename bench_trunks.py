@@ -4,7 +4,7 @@
   config 4   Resnet50FPN + AttentionDecoder (fpn50-attention-decoder.yaml), 3x64x256 lines (SURVEY.md D3)
 
 One "step" = forward + backward + Adam on one synthetic batch (per-GPU batch 32 = BASELINE's 256 over 8 GPUs; --batch overrides).
-bf16 compute on the repo's kernels: every convolution of trunk and head runs on the tcgen05 implicit-GEMM kernels
+bf16 compute on the repo's kernels: every convolution of trunk and head runs on the wgmma implicit-GEMM kernels
 (megreader_b200.conv_engine), the 2D-CTC head epilogue + loss on csrc/ctc2d_head.cu + csrc/ctc2d.cu, the attention decoder's recurrent
 loop on csrc/attn_decode.cu, the deformable units on csrc/dcn_tcgen05.cu, BatchNorm on the NHWC row kernels of csrc/nn_kernels.cu;
 ReLU / residual adds / pooling / interpolation are library (ATen) kernels.  The step is captured in CUDA graphs (MR_BENCH_EAGER=1: eager launches).
@@ -345,7 +345,7 @@ def run(args, peaks, ClockSampler, emit_json):
         "data": "synthetic",
         "config": {"workload": "%s, 3x%dx%d fp32 input, bf16 compute, Adam lr 1e-3" % (c["name"], c["hw"][0], c["hw"][1]),
                    "batch_per_gpu": batch, "global_batch": batch * world, "parallelism": "dp%d" % world,
-                   "l2": "3 rotating input batches; weights + gradients + Adam state (> 400 MB) and activations exceed the 126 MB L2"},
+                   "l2": "3 rotating input batches; weights + gradients + Adam state (> 400 MB) and activations exceed the 50 MB L2"},
         "e2e": {"value": lines / (ms_e2e / 1e3), "unit": "scenes/s" if cfg == 5 else "lines/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4,
                 "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": launches_per_step * args.steps, "final_loss": final_loss, "clocks": clocks,
@@ -354,14 +354,14 @@ def run(args, peaks, ClockSampler, emit_json):
     if rank == 0:
         out["roofline"] = conv_roofline(dev, peaks, cfg)
         out["cpu_baseline"] = cpu_arm(cfg, 2, 3)
-        out["stages"] = {"convolutions (trunk + head, %d layers)" % n_engine: "megreader_b200 tcgen05 implicit-GEMM kernels (fprop, dgrad, wgrad)",
+        out["stages"] = {"convolutions (trunk + head, %d layers)" % n_engine: "megreader_b200 wgmma implicit-GEMM kernels (fprop, dgrad, wgrad)",
                          "BatchNorm": "megreader_b200 NHWC row kernels (conv_engine.EngineBatchNorm2d: column statistics through block partials, "
                                       "row-tiled normalisation, fused backward)",
                          "ReLU / residual add / pooling / interpolation": "library (ATen, channels_last bf16)",
                          "head": ("megreader_b200 fused 2D-CTC epilogue + DP kernels" if cfg == 3 else
                                   "attention decoder: the 32-step loop and its backward through time = megreader_b200 persistent cooperative kernels (csrc/attn_decode.cu), hoisted encoder projection; weight-gradient products over the saved rows: library GEMMs" if cfg == 4 else
                                   "EAST head: 3x3 / 1x1 convolutions and the 2x2 stride-2 transposed convolutions (as 1x1 convolutions + depth-to-space) on the conv engine, losses library; "
-                                  "DCNv2 units: fused tcgen05 forward / weight-gradient / data-gradient kernels (csrc/dcn_tcgen05.cu)"),
+                                  "DCNv2 units: fused wgmma forward / weight-gradient / data-gradient kernels (csrc/dcn_tcgen05.cu)"),
                          "conv weight gradients": "side stream, joined at the end of the backward pass (conv_engine.WGRAD_SIDE_STREAM)"
                                                   if side_wgrad else "the backward's stream",
                          "Adam": "library (torch fused, capturable)", "launch": launch_mode}

@@ -1,4 +1,4 @@
-"""DCNv2 backward at the bench shapes: fused tcgen05 kernels vs the column-matrix + SGEMM route: python benchmarks/dcn_bwd.py"""
+"""DCNv2 backward at the bench shapes: fused wgmma kernels vs the column-matrix + SGEMM route: python benchmarks/dcn_bwd.py"""
 import os, sys, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from megreader_b200 import dcn

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (ours) vs cuBLAS on the CRNN conv GEMM shapes at batch 512 (fprop NT, dgrad NN, wgrad TN split-K)."""
+"""wgmma GEMM (ours) vs cuBLAS on the CRNN conv GEMM shapes at batch 512 (fprop NT, dgrad NN, wgrad TN split-K)."""
 import json
 import os
 import sys

@@ -1,5 +1,5 @@
 /*
- * megreader_b200 — C-ABI of the B200-native OCR hot path (drop-in for MegReader's native ops).
+ * megreader_b200 — C-ABI of the H100-native (sm_90a) OCR hot path (drop-in for MegReader's native ops).
  *
  * Plain pointers and sizes only: no torch / ATen types.  Every pointer is a DEVICE pointer unless
  * the name ends in `_host`.  `stream` is a cudaStream_t passed as void* (NULL = legacy default
@@ -138,7 +138,7 @@ int mr_dcn_forward_f32(const float *input, const float *weight, const float *bia
                        float *workspace, int64_t workspace_bytes, int B, int C, int H, int W, int Cout, int kh, int kw,
                        int sh, int sw, int ph, int pw, int dh, int dw, int group, int dg, void *stream);
 
-/* Fused forward (csrc/dcn_tcgen05.cu): the same result as mr_dcn_forward_f32 without a column matrix in HBM -- one tcgen05
+/* Fused forward (csrc/dcn_tcgen05.cu): the same result as mr_dcn_forward_f32 without a column matrix in HBM -- one wgmma
  * implicit GEMM whose A operand is the bilinear gather itself (bf16 hi/lo split, three MMAs per K block: fp32-level accuracy).
  * group = deformable_group = 1, C % 64 == 0, Cout % 128 == 0; workspace >= mr_dcn_fused_workspace_bytes(...) (NHWC copy of
  * the input + packed weights), 256-byte aligned.  Returns MR_ERR_UNSUPPORTED otherwise; mr_dcn_forward_f32 tries it first. */
@@ -149,7 +149,7 @@ int mr_dcn_forward_fused_f32(const float *input, const float *weight, const floa
                              int sh, int sw, int ph, int pw, int dh, int dw, int group, int dg, void *stream);
 
 /* Fused weight gradient (csrc/dcn_tcgen05.cu), the deform_conv_cuda.cpp:645-658 step (im2col + SGEMM per sample in the reference)
- * as one tcgen05 GEMM over the pixels whose B operand is the bilinear gather itself: grad_weight += scale * go (*) columns.
+ * as one wgmma GEMM over the pixels whose B operand is the bilinear gather itself: grad_weight += scale * go (*) columns.
  * Same eligibility as the fused forward; workspace >= mr_dcn_fused_wgrad_workspace_bytes(...).  mr_dcn_backward_f32 tries it first. */
 int64_t mr_dcn_fused_wgrad_workspace_bytes(int64_t B, int64_t C, int64_t H, int64_t W, int64_t Cout, int64_t Ho, int64_t Wo);
 int mr_dcn_wgrad_fused_f32(const float *input, const float *offset, int64_t offset_bstride, const float *mask, int64_t mask_bstride,
@@ -158,7 +158,7 @@ int mr_dcn_wgrad_fused_f32(const float *input, const float *offset, int64_t offs
                            int group, int dg, void *stream);
 
 /* Fused backward (csrc/dcn_tcgen05.cu): the weight gradient above plus the data gradient -- the deform_conv_cuda.cpp:611-614 SGEMM
- * (W^T . grad_output) and the K9 / K10 kernels (deform_conv_cuda_kernel.cu:634-766) as one tcgen05 kernel whose epilogue scatters
+ * (W^T . grad_output) and the K9 / K10 kernels (deform_conv_cuda_kernel.cu:634-766) as one wgmma kernel whose epilogue scatters
  * grad_input and reduces grad_offset / grad_mask, no column-gradient matrix in HBM.  group = deformable_group = 1, C % 128 == 0,
  * Cout % 128 == 0; workspace >= mr_dcn_fused_backward_workspace_bytes(...).  Same argument meaning as mr_dcn_backward_f32 (without
  * grad_bias); returns MR_ERR_UNSUPPORTED otherwise; mr_dcn_backward_f32 tries it first. */
@@ -236,7 +236,7 @@ int mr_gemm_batched(const void *A, const void *B, void *C, int64_t M, int64_t N,
                     int64_t ldc, int64_t strideA, int64_t strideB, int64_t strideC, int batch, int transA, int transB,
                     int in_dtype, int out_dtype, float alpha, float beta, void *stream);
 
-/* Hand-written Blackwell GEMM (tcgen05.mma + TMEM accumulators + TMA operand staging), bf16 in / fp32 accumulate.
+/* Hand-written Hopper GEMM (wgmma.mma_async with register accumulators + TMA operand staging), bf16 in / fp32 accumulate.
  * Same storage convention as mr_gemm; supported forms (transA,transB) = (0,1) and (1,0); optional per-column bias
  * and ReLU in the epilogue; beta = 1 accumulates atomically into fp32 C and enables split-K.  Returns
  * MR_ERR_UNSUPPORTED for shapes / alignments it does not cover (the caller then uses mr_gemm). */
@@ -244,7 +244,7 @@ int mr_gemm_tcgen05(const void *A, const void *B, void *C, int64_t M, int64_t N,
                     int64_t ldc, int transA, int transB, int out_dtype, const float *bias, int relu, float beta,
                     int splits, void *stream);
 
-/* Implicit-GEMM stride-1 convolution (nn.Conv2d of backbones/crnn.py:46-49) on NHWC bf16, tcgen05 + TMA + gathered
+/* Implicit-GEMM stride-1 convolution (nn.Conv2d of backbones/crnn.py:46-49) on NHWC bf16, wgmma + TMA + gathered
  * activation tiles: y[N*Ho*Wo, Cout] = conv(x[N,H,W,C], Wm[Cout, kh*kw*C]) (+bias, ReLU); C % 64 == 0.  With
  * flipped/transposed weights and padding (k-1-p) the same entry computes the input gradient. */
 int mr_conv_fprop_tcgen05(const void *x, const void *Wm, void *y, int N, int H, int W, int C, int Cout, int kh, int kw,
@@ -261,7 +261,7 @@ int mr_conv2d_wgrad_tcgen05(const void *dz, const void *x, float *dWm, int N, in
 int mr_conv_wgrad_tcgen05(const void *dz, const void *x, float *dWm, int N, int H, int W, int C, int Cout, int kh, int kw,
                           int ph, int pw, int splits, void *stream);
 
-/* Fused LSTM time steps on tcgen05 (recurrent GEMM + cell in one launch, both directions): gate columns are
+/* Fused LSTM time steps on wgmma (recurrent GEMM + cell in one launch, both directions): gate columns are
  * UNIT-MAJOR (column 4*j + g = gate g in {i,f,g,o} of hidden unit j), H % 64 == 0, bf16.  Every per-direction argument
  * is a HOST array of 2 device pointers.  fwd: gates[d] [B,4H] holds the x-projection on entry and the activated gates
  * on exit; bias[d] [4H] = b_ih + b_hh (unit-major); have_h = 0 on the first step.  bwd: dG_next[d] = gate gradients of
@@ -286,7 +286,7 @@ int mr_lstm_step_bwd_tcgen05(const void *const *dG_next, const void *const *Whh,
  * bwd:  dY [T, B, 2H] bf16 -> dG [2, T, B, 4H] bf16 gate gradients (the weight/input gradients are plain GEMMs on dG);
  *       WhhT = the recurrent weights TRANSPOSED, HOST array of 2 device pointers to [H, 4H] bf16 (unit-major columns).
  * MR_ERR_UNSUPPORTED when the CTA grid cannot be co-resident on this device or H exceeds the shared-memory budget
- * (fwd H <= 512, bwd H <= 256): callers then use the per-step entry points above. */
+ * (fwd H <= 384, bwd H <= 256: shared memory): callers then use the per-step entry points above. */
 int mr_lstm_seq_fwd_tcgen05(const void *const *Whh, void *G, const float *const *bias, float *C, void *Y,
                             unsigned *flags, int T, int B, int H, void *stream);
 int mr_lstm_seq_bwd_tcgen05(const void *const *WhhT, const void *G, const float *C, const void *dY, void *dG,
@@ -326,7 +326,7 @@ int mr_pack_labels(const unsigned char *text, const int64_t *offsets, int N, con
  *   mode 0: forward matrix [Cout, Kp], column (i*kw + j)*Cp + c, zero padded (Cp >= Cin, Kp >= kh*kw*Cp);
  *   mode 1: input-gradient matrix [Cin, kh*kw*Cout], taps flipped and (Cout,Cin) transposed.
  * mr_gate_rows_permute: nn.LSTM weight / bias rows [4H, cols] fp32 between the reference's gate-major order (i|f|g|o
- *   blocks) and the unit-major order of the tcgen05 LSTM kernels; `b` (nullable) is added (b_ih + b_hh). */
+ *   blocks) and the unit-major order of the wgmma LSTM kernels; `b` (nullable) is added (b_ih + b_hh). */
 int mr_conv_weight_pack(const float *w, int Cout, int Cin, int kh, int kw, int Cp, int Kp, int mode, int dtype, void *out,
                         void *stream);
 int mr_gate_rows_permute(const float *a, const float *b, int H, int cols, int inverse, int dtype, void *out, void *stream);

@@ -1,4 +1,4 @@
-"""megreader_b200 — B200-native (sm_100a) rebuild of MegReader's recognition hot path.
+"""megreader_b200 — H100-native (sm_90a) rebuild of MegReader's recognition hot path.
 
 Host code is Python/PyTorch (device memory, streams, torch.distributed); all arithmetic on the
 path runs in hand-written CUDA reached through the C-ABI in include/megreader_b200.h

@@ -1,8 +1,8 @@
-"""Build the C-ABI library in-tree with nvcc for sm_100a (no torch headers involved).
+"""Build the C-ABI library in-tree with nvcc for sm_90a (no torch headers involved).
 
     python -m megreader_b200.build          # -> megreader_b200/libmegreader_b200.so
 
-nvcc cross-compiles without a GPU; the .so travels to the GPU box with the gpurun snapshot.
+nvcc cross-compiles without a GPU.
 """
 import glob
 import os
@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(CSRC, "_obj")
 SO = os.path.join(HERE, "libmegreader_b200.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 

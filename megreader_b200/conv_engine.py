@@ -1,4 +1,4 @@
-"""General 2-D convolution on the tcgen05 implicit-GEMM kernels (csrc/gemm_tcgen05.cu) as an autograd Function, and the module
+"""General 2-D convolution on the wgmma implicit-GEMM kernels (csrc/gemm_tcgen05.cu) as an autograd Function, and the module
 swap that puts the reference-named trunks on it.
 
     conv2d(x, weight, bias, stride, padding, dilation)            x, result: (N, C, H, W) bf16 in channels_last memory
@@ -188,7 +188,7 @@ class _StemFn(torch.autograd.Function):
         Cout, Cin, kh, kw, K, has_bias, wdtype = ctx.geo
         dz = dy.permute(0, 2, 3, 1).reshape(-1, Cout).to(torch.bfloat16).contiguous()
         # [Cout, Kp] = dz^T A: a tiny output over a reduction as long as the batch has pixels (524,288 rows at 8 x 512 x 512) --
-        # split-K over up to 128 CTAs, fp32 atomics into the zero-filled result (one CTA took 1.8 ms there, profiles/r2_cfg5_launch_top.txt)
+        # split-K over up to 128 CTAs, fp32 atomics into the zero-filled result
         splits = max(1, min(128, dz.size(0) // 4096))
         if splits > 1:
             dWm = torch.zeros((Cout, A.size(1)), dtype=torch.float32, device=dz.device)
@@ -201,7 +201,7 @@ class _StemFn(torch.autograd.Function):
 
 
 class EngineConv2d(nn.Conv2d):
-    """nn.Conv2d whose arithmetic runs on megreader_b200's tcgen05 kernels (same parameters, same state-dict keys)."""
+    """nn.Conv2d whose arithmetic runs on megreader_b200's wgmma kernels (same parameters, same state-dict keys)."""
 
     def forward(self, x):
         if self.groups != 1 or self.padding_mode != "zeros" or isinstance(self.padding, str):
@@ -274,7 +274,7 @@ class EngineBatchNorm2d(nn.BatchNorm2d):
 
 
 class EngineConvTranspose2d(nn.ConvTranspose2d):
-    """nn.ConvTranspose2d with kernel = stride = 2 x 2 (the up-sampling layers of decoders/east.py:20-21) on the tcgen05 convolution
+    """nn.ConvTranspose2d with kernel = stride = 2 x 2 (the up-sampling layers of decoders/east.py:20-21) on the wgmma convolution
     kernels: such a layer is a 1 x 1 convolution to 4 * C_out channels -- one output channel block per (row, column) offset inside the
     2 x 2 cell -- followed by a depth-to-space rearrangement.  The weight re-layout and the rearrangement are framework views / copies,
     so autograd carries the gradients back to the reference-shaped parameters.  Other geometries use the library implementation."""

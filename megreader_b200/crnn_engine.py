@@ -17,14 +17,13 @@ from . import ctc1d
 from . import nnops as ops
 
 _COMPUTE_DTYPE = torch.float32
-# bf16 mode: convolutions with C % 64 == 0 run as tcgen05 implicit GEMMs (csrc/gemm_tcgen05.cu); False routes them
+# bf16 mode: convolutions with C % 64 == 0 run as wgmma implicit GEMMs (csrc/gemm_tcgen05.cu); False routes them
 # through im2col + cuBLAS (kept for A/B comparison in benchmarks)
 USE_TCGEN05 = __import__("os").environ.get("MEGREADER_B200_TCGEN05", "1") != "0"
-# Fused tcgen05 LSTM time steps (recurrent GEMM + cell in one launch).  Correct (tests/test_nn_kernels_gpu.py) but
-# measured 0.7 ms/step SLOWER at batch 512 than cuBLAS strided-batched GEMM + cell kernel (per-launch TMEM/barrier
-# set-up dominates a 4-k-block GEMM), so it is opt-in.
-# BiLSTM recurrence on the bf16 path: "seq" = one persistent tcgen05 launch per layer and pass (csrc/lstm_seq_tcgen05.cu),
-# "step" = one fused tcgen05 launch per time step, "cublas" = strided-batched cuBLAS GEMM + cell kernel per step.
+# Fused wgmma LSTM time steps (recurrent GEMM + cell in one launch).  Correct (tests/test_nn_kernels_gpu.py) but
+# the per-launch barrier set-up dominates a 4-k-block GEMM, so it is opt-in.
+# BiLSTM recurrence on the bf16 path: "seq" = one persistent wgmma launch per layer and pass (csrc/lstm_seq_tcgen05.cu),
+# "step" = one fused wgmma launch per time step, "cublas" = strided-batched cuBLAS GEMM + cell kernel per step.
 LSTM_MODE = __import__("os").environ.get("MEGREADER_B200_LSTM", "seq")
 if __import__("os").environ.get("MEGREADER_B200_LSTM_FUSED", "0") == "1":     # older switch
     LSTM_MODE = "step"
@@ -129,7 +128,7 @@ class _BackboneFn(torch.autograd.Function):
             Wm = _weight_matrix(conv.weight, C, Kp, dtype)
             implicit = USE_TCGEN05 and dtype == torch.bfloat16 and C % 64 == 0
             if implicit:
-                # tcgen05 implicit GEMM: activation tiles are gathered straight into swizzled smem, no im2col in HBM
+                # wgmma implicit GEMM: activation tiles are gathered straight into swizzled smem, no im2col in HBM
                 z, Ho, Wo = ops.conv_fprop_tc(a, Wm, kh, kw, ph, pw)
                 col = None
             else:
@@ -330,7 +329,7 @@ def _unit_major_perm(H, dev):
 
 
 def _bilstm_forward_fused(X, params, training):
-    """bf16 path: each time step is ONE tcgen05 launch (recurrent GEMM + cell, both directions), csrc/gemm_tcgen05.cu."""
+    """bf16 path: each time step is ONE wgmma launch (recurrent GEMM + cell, both directions), csrc/gemm_tcgen05.cu."""
     dtype = torch.bfloat16
     T, N, I = X.shape
     w_ih, w_hh = [params[0], params[4]], [params[1], params[5]]
@@ -421,7 +420,7 @@ def _bilstm_backward_fused(dE, sv):
         if d == 0 or ops.GEMM_BACKEND != "tc":
             ops.gemm(dG2, sv["Wih"][d], out=dX, beta=0.0 if d == 0 else 1.0)
         else:
-            dX.add_(ops.gemm(dG2, sv["Wih"][d]))       # tcgen05 kernel: no bf16 accumulate form -> own GEMM + one add
+            dX.add_(ops.gemm(dG2, sv["Wih"][d]))       # wgmma kernel: no bf16 accumulate form -> own GEMM + one add
     return dX.view(T, N, I), grads + [dWemb, dbemb]
 
 

@@ -28,10 +28,10 @@ int ensure_dyn_smem(const void *func, size_t bytes, const char *where) {
 int sm_count() {
     static std::atomic<int> cache[16];
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 16) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 16) return 132;
     int v = cache[dev].load(std::memory_order_relaxed);
     if (v <= 0) {
-        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 148;
+        if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
         cache[dev].store(v, std::memory_order_relaxed);
     }
     return v;

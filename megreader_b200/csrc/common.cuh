@@ -1,4 +1,4 @@
-// Shared helpers for the megreader_b200 C-ABI library (sm_100a only).
+// Shared helpers for the megreader_b200 C-ABI library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cublas_v2.h>

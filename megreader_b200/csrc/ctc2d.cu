@@ -1,4 +1,4 @@
-// 2D-CTC loss for sm_100a — forward (log_alpha + nll), backward (gradient), and the training pair
+// 2D-CTC loss for sm_90a — forward (log_alpha + nll), backward (gradient), and the training pair
 // (forward_train + backward_apply).  Replaces the reference's four SIMT kernels
 // (ops/ctc_2d/csrc/cuda/ctc2d_cuda_kernel.cu:54-211 K1, :254-368 K2, :427-517 K3) — not a port:
 //
@@ -34,8 +34,7 @@ template <> struct Lim<float> { static __device__ __forceinline__ float ninf() {
 template <> struct Lim<double> { static __device__ __forceinline__ double ninf() { return -(double)INFINITY; } };
 
 // fast path: one FMUL + one MUFU each (ex2/lg2.approx.ftz).  __expf/__logf without -use_fast_math expand to
-// denormal-safe sequences (FSETP + 2 extra FMUL) that were 24 % of all issued instructions in the DP kernel
-// (profiles/ctc2d_dpwarp_r1_summary.md); flushing results below 1.2e-38 to zero is harmless in a log-sum-exp.
+// denormal-safe sequences (FSETP + 2 extra FMUL), a large share of the DP kernel's instructions; flushing results below 1.2e-38 to zero is harmless in a log-sum-exp.
 __device__ __forceinline__ float ex2_ftz(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float lg2_ftz(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 template <bool FAST> __device__ __forceinline__ float ex(float x) { return FAST ? ex2_ftz(x * 1.4426950408889634f) : expf(x); }
@@ -108,8 +107,7 @@ __device__ __forceinline__ StateCtx make_ctx(const Geo &q, int b0, int Gv, const
 // The [H, G*C] slab of log_probs for column t is prefetched kStages-1 columns ahead with cp.async;
 // it feeds both Q[t] and the expansion, so HBM sees every byte of log_probs exactly once.
 // All per-thread addressing (copy plan, output pointer, gather offset) is hoisted out of the column
-// loop: the first version of this kernel spent 60 % of its issue slots on index arithmetic
-// (profiles/ctc2d_r1a_summary.md).
+// loop: index arithmetic otherwise takes most of the issue slots.
 // ------------------------------------------------------------------------------------------------
 constexpr int kPlan = 4;  // cp.async chunks per thread per column held in registers
 
@@ -569,8 +567,7 @@ __global__ void ctc2d_dp_kernel(Geo q, const real *__restrict__ lp, const int64_
 // ------------------------------------------------------------------------------------------------
 // Warp-per-sample DP kernel (fp32, fast math), third revision.  Same phases as ctc2d_dp_kernel, but:
 //   * the two sweeps of a sample run inside ONE warp, states in registers (lane L holds states [L*NS, L*NS+NS)),
-//     neighbours by warp shuffle, no block barrier inside the 2*T steps (ncu on the block version: barrier stalls
-//     6.6 per issued instruction, issue slots 32 % busy -- profiles/ctc2d_dpblock_r1_summary.md);
+//     neighbours by warp shuffle, no block barrier inside the 2*T steps (the block version stalls on its barriers);
 //   * NS is chosen PER SAMPLE from its target length (2L+1 <= 32 -> one state per lane), so short targets do a third
 //     of the work of the padded S = 32 layout;
 //   * everything is in log2 units (Q2 = log2(e) * Q): no FMUL around the MUFUs, and the log-sum-exp of three terms
@@ -799,8 +796,7 @@ ctc2d_dp_warp_kernel(Geo q, const float *__restrict__ lp, const int64_t *__restr
 
 // ------------------------------------------------------------------------------------------------
 // Warp-per-sample DP kernel, FOURTH revision (round 2; fp32 fast math; modes GRAD and FAC; S <= 32, C <= 64).
-// ncu on v3: ~12 k warp-instructions per sample at IPC 1.6 with 16 warps per SM -- every phase ran as one dependent
-// instruction chain.  What changed (profiles/ctc2d_dp4_r2_summary.md has the per-phase instruction counts):
+// In the third revision every phase ran as one dependent instruction chain.  What changed:
 //   * the forward and the backward sweep of a sample run INTERLEAVED in the same warp: two independent dependency chains
 //     per iteration, and T+1 instead of 2T chain steps.  The forward chain covers columns 0..m, the backward chain
 //     Tb-1..m (m = Tb/2); they meet at column m, where  -nll = LSE_s(R[m,s] + Rb[m,s] + Q[m,l'_s])  (every path crosses

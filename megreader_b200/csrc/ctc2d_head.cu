@@ -32,7 +32,7 @@ __device__ __forceinline__ float ex2f(float x) { float y; asm("ex2.approx.ftz.f3
 __device__ __forceinline__ float lg2f(float x) { float y; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 constexpr float kLog2e = 1.4426950408889634f, kLn2 = 0.6931471805599453f;
 // base + i * stride_bytes with a 32 x 32 -> 64-bit multiply-add: ONE IMAD.WIDE.U32 per address (the plain pointer + int form
-// cost 5-7 integer instructions per access in these kernels: 55 % of all issued instructions, profiles/ctc2d_head_r2_summary.md)
+// costs 5-7 integer instructions per access, which dominated the instruction count of these kernels)
 __device__ __forceinline__ const float *at(const float *base, unsigned i, unsigned stride_bytes) {
     return reinterpret_cast<const float *>(reinterpret_cast<const char *>(base) + (uint64_t)i * stride_bytes);
 }
@@ -99,7 +99,7 @@ __device__ __forceinline__ void column_max_sum(const float *col, int C, float &m
 __device__ __forceinline__ void load_nchw_tile(const HeadGeo &g, const float *__restrict__ z, int n0, int h, int w0,
                                                float *tile) {
     // batches of 8 independent loads per thread before the first shared-memory store: a load -> store loop body makes
-    // every iteration wait for its own load (38 serialised memory latencies per block; measured 28-46 us per block)
+    // every iteration wait for its own load (38 serialised memory latencies per block)
     const int w = threadIdx.x & 31, r0 = threadIdx.x >> 5;
     const int rows = g.NT * g.C;
     constexpr int RS = kThreads / 32, B = 20;           // 8 samples x 38 classes = 304 rows = 2 batches per thread
@@ -266,8 +266,8 @@ __global__ void ctc2d_head_mask_bwd_kernel(int N, int H, int W, const float *__r
 // =====================================================================================================
 // Round-2 kernels: one WARP per slab (sample n, height h, 32 columns), lane = column.
 //
-// ncu / timing of the block-tile kernels above (profiles/ctc2d_head_micro_r1.jsonl): 31 % (forward) and 17 % (backward)
-// of the HBM roofline -- three barrier-separated phases per block, ~1000 instructions per thread around 4-byte accesses.
+// The block-tile kernels above run three barrier-separated phases per block and ~1000 instructions per thread around
+// 4-byte accesses, far from the HBM roofline.
 // Here a lane keeps ITS column's C class logits in registers: every global read of the NCHW side is a coalesced 128-byte
 // row straight into registers (C + 2H independent loads in flight per lane, no staging), the softmax over C and the
 // log-softmax of the mask column are register arithmetic, and only the (T,H,N,C) side -- whose contiguous direction is

@@ -1,4 +1,4 @@
-// Deformable convolution v1 / v2 (modulated) for sm_100a, fp32, NCHW — replaces the reference extension
+// Deformable convolution v1 / v2 (modulated) for sm_90a, fp32, NCHW — replaces the reference extension
 // `deform_conv_cuda` (assets/ops/dcn/src/deform_conv_cuda.cpp:151-695, deform_conv_cuda_kernel.cu K5-K10).
 //
 // Not a port.  The reference loops over the batch on the host (1 im2col launch + G GEMMs per sample,
@@ -210,7 +210,7 @@ int fill_geo(DcnGeo &g, int B, int C, int H, int W, int Cout, int kh, int kw, in
 
 int grid_for(int64_t threads_total, int block) {
     int64_t blocks = ceil_div(threads_total, block);
-    const int64_t cap = 148 * 32;
+    const int64_t cap = (int64_t)mr::sm_count() * 32;
     return (int)(blocks < 1 ? 1 : (blocks > cap ? cap : blocks));
 }
 
@@ -218,7 +218,7 @@ int pick_csplit(const DcnGeo &g, int nb) {
     // enough sampling points to fill the chip? otherwise slice the channel loop
     const int64_t pts = (int64_t)nb * g.dg * g.K * g.P;
     int cs = 1;
-    while (pts * cs < 148 * 2048 * 2 && cs * 2 <= g.cpg && cs < 32) cs *= 2;
+    while (pts * cs < mr::sm_count() * 2048 * 2 && cs * 2 <= g.cpg && cs < 32) cs *= 2;
     return cs;
 }
 
@@ -239,7 +239,7 @@ int mr_dcn_forward_f32(const float *input, const float *weight, const float *bia
     if (rc) return rc;
     if (B == 0) return MR_OK;
     if (!input || !weight || !offset || !output || !workspace) return MR_ERR_NULL_POINTER;
-    // fused tcgen05 implicit GEMM (csrc/dcn_tcgen05.cu) when the shape qualifies and the workspace holds its scratch
+    // fused wgmma implicit GEMM (csrc/dcn_tcgen05.cu) when the shape qualifies and the workspace holds its scratch
     rc = mr_dcn_forward_fused_f32(input, weight, bias, offset, offset_bstride, mask, mask_bstride, output, workspace,
                                   workspace_bytes, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg, stream);
     if (rc != MR_ERR_UNSUPPORTED) return rc;
@@ -300,14 +300,14 @@ int mr_dcn_backward_f32(const float *input, const float *weight, const float *of
     const float one = 1.f, zero = 0.f;
     const bool want_data = grad_input || grad_offset || grad_mask;
     bool wgrad_done = false;
-    // everything but grad_bias on the fused tcgen05 kernels when the shape allows (csrc/dcn_tcgen05.cu)
+    // everything but grad_bias on the fused wgmma kernels when the shape allows (csrc/dcn_tcgen05.cu)
     rc = mr_dcn_backward_fused_f32(input, weight, offset, offset_bstride, mask, mask_bstride, grad_output, grad_input, grad_weight,
                                    grad_offset, grad_offset_bstride, grad_mask, grad_mask_bstride, weight_grad_scale, workspace,
                                    workspace_bytes, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg, stream);
     if (rc != MR_OK && rc != MR_ERR_UNSUPPORTED) return rc;
     const bool fused_all = rc == MR_OK;
     if (grad_weight && !fused_all) {
-        // fused tcgen05 weight gradient (csrc/dcn_tcgen05.cu): uses the workspace first; the loop below reuses it afterwards
+        // fused wgmma weight gradient (csrc/dcn_tcgen05.cu): uses the workspace first; the loop below reuses it afterwards
         rc = mr_dcn_wgrad_fused_f32(input, offset, offset_bstride, mask, mask_bstride, grad_output, grad_weight, weight_grad_scale,
                                     workspace, workspace_bytes, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg, stream);
         if (rc == MR_OK) wgrad_done = true;

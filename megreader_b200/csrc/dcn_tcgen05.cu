@@ -1,28 +1,28 @@
-// Deformable convolution v1 / v2 FORWARD as ONE fused implicit GEMM on tcgen05 (round 2).
+// Deformable convolution v1 / v2 FORWARD as ONE fused implicit GEMM on wgmma (round 2).
 //
 //   out[b, co, p] = sum_{k, c} W[co, c, k] * mask[b, k, p] * bilinear(x[b, c], pos(b, k, p))  (+ bias)
 //   (modulated_deform_conv_cuda_forward, assets/ops/dcn/src/deform_conv_cuda.cpp:486-564; K8 deform_conv_cuda_kernel.cu:569-632)
 //
-// Round 1 (csrc/dcn.cu) wrote the 9x column matrix to HBM and multiplied it with an fp32 SIMT SGEMM: 319 us for
-// B = 8, C = 128 @ 64 x 64, half of it in the GEMM (profiles/dcn_r1_summary.md).  Here the column matrix never exists:
+// The unfused path (csrc/dcn.cu) writes the 9x column matrix to HBM and multiplies it with an fp32 GEMM.  Here the column
+// matrix never exists:
 //
 //   GEMM view      M = output pixels (128-row tiles inside a sample), N = Cout, K = taps x channels, K index = (cb * taps + k) * 64 + cl
 //                  (a 64-wide K block is ONE tap and 64 consecutive channels; the nine taps of a channel block are consecutive K
 //                  blocks, so their overlapping sampling positions are served by L1).
 //   A operand      produced on the fly: 512 producer threads (8 lanes per pixel row, 2 rows each) read the four corners from an NHWC copy
 //                  of the input: a warp-wide float4 gather is 4 x 128 contiguous bytes; 16 gathers per thread are in flight, blend, fold the
-//                  modulation mask in, and store bf16 into the 128-byte-swizzled K-major tile that tcgen05.mma reads.
+//                  modulation mask in, and store bf16 into the 128-byte-swizzled K-major tile that wgmma.mma_async reads.
 //   precision      fp32 parity (1e-4, against the reference's own kernels) with tensor cores: every value is split
 //                  v = hi + lo (two bf16), and D += Ah Wh + Ah Wl + Al Wh -- three bf16 MMAs per K block, error ~2^-17 relative
-//                  (the dropped Al Wl term), fp32 accumulation in TMEM.
+//                  (the dropped Al Wl term), fp32 accumulation in the MMA warpgroup's registers.
 //   B operand      weights re-packed per call to [Cout][k * C + c] bf16 (hi and lo), tiles by 2-D TMA.
-//   epilogue       TMEM -> registers -> NCHW output: a warp's 32 lanes are 32 consecutive pixels of one output channel, so
+//   epilogue       accumulator tile (shared memory) -> registers -> NCHW output: a warp's 32 lanes are 32 consecutive pixels of one output channel, so
 //                  every store instruction is one coalesced 128-byte row; bias added on the way.
 //
 // Requirements of this path: group = 1, deformable_group = 1, C % 64 == 0, Cout % 128 == 0 (the ResNet-50 DCN units of
 // backbones/resnet.py:136-165 are C = Cout = 128 / 256 / 512); anything else uses the round-1 kernels in dcn.cu.
 // The offset / mask indexing quirk (flat (Ho,Wo) strides inside a possibly larger per-sample slab, SURVEY.md App. B2.1) is kept.
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 #include <math.h>
 #include <stdlib.h>
 #include <algorithm>
@@ -45,12 +45,13 @@ struct DcnSmem {
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
     static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
-    static constexpr int TAP_OFF = BAR_OFF + 128;             // barriers + TMEM slot live in the first 128 bytes
+    static constexpr int TAP_OFF = BAR_OFF + 128;             // barriers live in the first 128 bytes
     static constexpr int total(int taps) { return TAP_OFF + BM * taps * 24 + 1024; }   // + tap table (16 + 8 bytes / entry)
 };
 
 constexpr int kProducerThreads = 512;      // 16 warps x (4 rows x 8 channel lanes) x 2 row quads = 128 rows
-constexpr int kDcnThreads = 64 + kProducerThreads;
+constexpr int kDcnMma0 = 640;                 // producer warps end at 576; padded to a warpgroup boundary
+constexpr int kDcnThreads = kDcnMma0 + kMmaThreads;
 
 __device__ __forceinline__ void mbar_arrive_cta(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
@@ -65,7 +66,6 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
     uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
     uint64_t *empty = full + STAGES;
     uint64_t *tmem_full = empty + STAGES;
-    uint32_t *tmem_slot = (uint32_t *)(tmem_full + 1);
     float4 *tapw = (float4 *)(smem + L::TAP_OFF);             // [taps][128] bilinear weights
     uint2 *tapc = (uint2 *)(tapw + BM * a.kh * a.kw);         // [taps][128] clamped corner rows / columns
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -84,12 +84,48 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
         mbar_init(tmem_full, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, BN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    float *acc_tile = (float *)smem;                         // laid over the drained operand ring when the K loop is over
 
+    // 768 threads leave 80 registers each: the MMA warpgroup takes what its 128 accumulator registers need from the others
+    if (threadIdx.x >= kDcnMma0) {
+        reg_inc<160>();
+        // ------------------------------------------------------------ MMA warpgroup: D += Ah Wh + Ah Wl + Al Wh
+        static_assert(BN == 128, "one warpgroup holds a 128 x 128 accumulator");
+        const int mt = threadIdx.x - kDcnMma0;
+        AccTile<BN> acc;
+        uint64_t *pending = nullptr;
+        for (int i = 0; i < nkb; ++i) {
+            const int s = i % STAGES;
+            mbar_wait(full + s, (i / STAGES) & 1);
+            const uint32_t ah = smem_u32(smem + s * L::STAGE_BYTES);
+            const uint32_t al = ah + L::A_BYTES;
+            const uint32_t bh = al + L::A_BYTES;
+            const uint32_t bl = bh + L::B_BYTES;
+            wgmma_fence();
+#pragma unroll
+            for (int pass = 0; pass < 3; ++pass) {
+                const uint32_t aa = pass == 2 ? al : ah, bb = pass == 1 ? bl : bh;
+#pragma unroll
+                for (int k = 0; k < BK / UMMA_K; ++k)
+                    acc.template mma_halves<0, 0>(make_desc(aa + k * 32, 16, 1024), make_desc(aa + 64 * 128 + k * 32, 16, 1024),
+                                                  make_desc(bb + k * 32, 16, 1024), make_desc(bb + 64 * 128 + k * 32, 16, 1024),
+                                                  (i | pass | k) != 0);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (pending && mt == 0) mbar_arrive_cta(pending);
+            pending = empty + s;
+        }
+        wgmma_wait<0>();
+        if (pending && mt == 0) mbar_arrive_cta(pending);
+        mma_group_sync();
+        acc.store(acc_tile, mt);
+        mma_group_sync();
+        if (mt == 0) mbar_arrive_cta(tmem_full);
+        return;
+    }
+    reg_dec<64>();
     if (warp == 0) {
         // ------------------------------------------------------------ weight tiles (hi and lo) by TMA
         if (elect_one()) {
@@ -102,38 +138,12 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
                 tma_load_2d(&tmWl, full + s, st + L::B_BYTES, i * BK, n0);
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------ MMA issuer: D += Ah Wh + Ah Wl + Al Wh
-        constexpr uint32_t idesc = make_idesc(BM, BN, 0, 0);
-        for (int i = 0; i < nkb; ++i) {
-            const int s = i % STAGES;
-            mbar_wait(full + s, (i / STAGES) & 1);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t ah = smem_u32(smem + s * L::STAGE_BYTES);
-                const uint32_t al = ah + L::A_BYTES;
-                const uint32_t bh = al + L::A_BYTES;
-                const uint32_t bl = bh + L::B_BYTES;
-#pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k)
-                    umma_bf16(tmem_base, make_desc(ah + k * 32, 16, 1024), make_desc(bh + k * 32, 16, 1024), idesc, (i | k) != 0);
-#pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k)
-                    umma_bf16(tmem_base, make_desc(ah + k * 32, 16, 1024), make_desc(bl + k * 32, 16, 1024), idesc, 1);
-#pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k)
-                    umma_bf16(tmem_base, make_desc(al + k * 32, 16, 1024), make_desc(bh + k * 32, 16, 1024), idesc, 1);
-                umma_commit(empty + s);
-                if (i == nkb - 1) umma_commit(tmem_full);
-            }
-            __syncwarp();
-        }
-    } else {
+    } else if (warp >= 2 && threadIdx.x < 64 + kProducerThreads) {
         // ------------------------------------------------------------ producers: bilinear gather -> swizzled bf16 tiles
         // Thread mapping: 8 lanes share a pixel row and split its 64 channels (lane j: channels 4j..4j+3 and 32+4j..32+4j+3),
         // 4 rows per warp instruction, 2 such row quads per warp.  A warp-wide float4 gather therefore touches 4 x 128
         // contiguous bytes (4 L1 wavefronts); with lanes = 32 different pixels it was 32 separate half-used sectors and
-        // the kernel was bound by the L1 data stage (ncu: l1tex 78 % busy, 27 sectors / request, profiles/dcn_r2_summary.md).
+        // the gathers were bound by the L1 data stage.
         const int pwp = warp - 2;                             // producer warp 0..15
         const int sub = lane >> 3, j = lane & 7;
         struct Row { const float4 *q1, *q2, *q3, *q4; float w1, w2, w3, w4; };
@@ -229,23 +239,22 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
                         asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(ah_s + (uint32_t)L::A_BYTES + o), "r"(lo.x), "r"(lo.y) : "memory");
                     }
                 }
-                fence_proxy_async();                          // generic-proxy smem writes -> visible to tcgen05
+                fence_proxy_async();                          // generic-proxy smem writes -> visible to wgmma
                 mbar_arrive_cta(full + s);
             }
         }
-        // ------------------------------------------------------------ epilogue: TMEM -> NCHW (+ bias); 4 warps per TMEM quarter
-        const int q = warp & 3;                               // TMEM lane quarter this warp may access
-        const int part = (warp - 2) >> 2;                     // which quarter of the BN columns (4 warps share a TMEM quarter)
+        // ------------------------------------------------------------ epilogue: accumulator tile -> NCHW (+ bias); 4 warps per 32-row quarter
+        const int q = warp & 3;                               // 32-row quarter of the tile this warp stores
+        const int part = (warp - 2) >> 2;                     // which quarter of the BN columns (4 warps share a row quarter)
         const int er = q * 32 + lane;
         const int ey = ty0 + (er >> 4), ex = tx0 + (er & 15);
         const int prow = (ey < a.Ho && ex < a.Wo) ? ey * a.Wo + ex : a.P;
         mbar_wait(tmem_full, 0);
-        tc_fence_after();
         float *ob = a.out + ((int64_t)b * a.Cout + n0) * a.P + prow;
 #pragma unroll 1
         for (int c = part * (BN / 128); c < (part + 1) * (BN / 128); ++c) {
             uint32_t rr[32];
-            tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), rr);
+            acc_ld<32>(acc_tile, AccTile<BN>::LD, q * 32, c * 32, rr);
             if (prow < a.P) {
 #pragma unroll
                 for (int j = 0; j < 32; ++j) {
@@ -256,12 +265,6 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
                 }
             }
         }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, BN);
     }
 }
 
@@ -303,7 +306,6 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
     uint64_t *empty = full + STAGES;
     uint64_t *a_full = empty + STAGES, *a_empty = a_full + 1;  // TMA operand, single buffer
     uint64_t *tmem_full = a_empty + 1;
-    uint32_t *tmem_slot = (uint32_t *)(tmem_full + 1);
     float4 *tapw_all = (float4 *)(smem + L::TAP_OFF);         // [STAGES][128]
     uint2 *tapc_all = (uint2 *)(tapw_all + STAGES * BM);      // [STAGES][128]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -311,7 +313,7 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
     const int cc = kb / (a.kh * a.kw), k = kb - cc * (a.kh * a.kw);
     const int co0 = blockIdx.z * BM;
     const int nt = (a.ntiles - (int)blockIdx.y + a.splits - 1) / a.splits;      // pixel tiles of this CTA: y, y + splits, ...
-    constexpr uint32_t BN = 64;
+    constexpr int BN = 64;
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmGh);
@@ -321,11 +323,8 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
         mbar_init(tmem_full, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, BN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    float *acc_tile = (float *)smem;                         // laid over the drained operand ring when the loop is over
 
     if (warp == 0) {
         if (elect_one()) {
@@ -341,33 +340,40 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                 tma_load_2d(&tmGl, a_full, st + L::A_BYTES + BM * 128, 64, row);
             }
         }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = make_idesc(BM, BN, 0, 1);              // A K-major (pixels contiguous), B MN-major (kc contiguous)
+    } else if (threadIdx.x >= kDcnMma0) {
+        // A K-major (pixels contiguous), B MN-major (kc contiguous)
+        const int mt = threadIdx.x - kDcnMma0;
+        AccTile<BN> acc;
         for (int i = 0; i < nt; ++i) {
             const int s = i % STAGES;
             mbar_wait(full + s, (i / STAGES) & 1);
             mbar_wait(a_full, i & 1);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t bh = smem_u32(smem + s * 2 * L::B_BYTES);
-                const uint32_t bl = bh + L::B_BYTES;
-                const uint32_t ah = smem_u32(smem + L::A_OFF);
-                const uint32_t al = ah + L::A_BYTES;
+            const uint32_t bh = smem_u32(smem + s * 2 * L::B_BYTES);
+            const uint32_t bl = bh + L::B_BYTES;
+            const uint32_t ah = smem_u32(smem + L::A_OFF);
+            const uint32_t al = ah + L::A_BYTES;
+            wgmma_fence();
 #pragma unroll
-                for (int pass = 0; pass < 3; ++pass) {
-                    const uint32_t aa = pass == 2 ? al : ah, bb = pass == 1 ? bl : bh;       // Ah Bh, Ah Bl, Al Bh
+            for (int pass = 0; pass < 3; ++pass) {
+                const uint32_t aa = pass == 2 ? al : ah, bb = pass == 1 ? bl : bh;       // Ah Bh, Ah Bl, Al Bh
 #pragma unroll
-                    for (int j = 0; j < BM / UMMA_K; ++j)                                     // 8 steps of 16 pixels
-                        umma_bf16(tmem_base, make_desc(aa + (j >> 2) * (BM * 128) + (j & 3) * 32, 16, 1024),
-                                  make_desc(bb + j * 2048, BM * 128, 1024), idesc, (i | pass | j) != 0);
+                for (int j = 0; j < BM / UMMA_K; ++j) {                                   // 8 steps of 16 pixels
+                    const uint32_t ak = aa + (j >> 2) * (BM * 128) + (j & 3) * 32;
+                    acc.mma<0, 1>(make_desc(ak, 16, 1024), make_desc(ak + 64 * 128, 16, 1024), make_desc(bb + j * 2048, BM * 128, 1024),
+                                  (i | pass | j) != 0);
                 }
-                umma_commit(empty + s);
-                umma_commit(a_empty);
-                if (i == nt - 1) umma_commit(tmem_full);
             }
-            __syncwarp();
+            wgmma_commit();
+            wgmma_wait<0>();
+            if (mt == 0) { mbar_arrive_cta(empty + s); mbar_arrive_cta(a_empty); }
         }
-    } else {
+        if (nt > 0) {
+            mma_group_sync();
+            acc.store(acc_tile, mt);
+            mma_group_sync();
+            if (mt == 0) mbar_arrive_cta(tmem_full);
+        }
+    } else if (warp >= 2 && threadIdx.x < 64 + kProducerThreads) {
         const int pwp = warp - 2;
         const int sub = lane >> 3, j = lane & 7;
         const int ptid = threadIdx.x - 64;
@@ -471,26 +477,19 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
             if (prep) tap_store(gt + a.splits, (i + 1) & 1, noh, now, nm);
             asm volatile("bar.sync 1, %0;" ::"n"(kProducerThreads) : "memory");
         }
-        // ---- epilogue: D[co][kc] -> gw[co][c][k] (fp32 atomics; 4 warps per TMEM quarter, 16 columns each)
+        // ---- epilogue: D[co][kc] -> gw[co][c][k] (fp32 atomics; 4 warps per row quarter, 16 columns each)
         const int q = warp & 3, part = (warp - 2) >> 2;
         const int co = co0 + q * 32 + lane;
         if (nt > 0) {
             mbar_wait(tmem_full, 0);
-            tc_fence_after();
             uint32_t rr[16];
-            tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(part * 16), rr);
+            acc_ld<16>(acc_tile, AccTile<BN>::LD, q * 32, part * 16, rr);
             if (co < a.Cout) {
                 float *gp = a.gw + ((int64_t)co * a.C + cc * BK + part * 16) * (a.kh * a.kw) + k;
 #pragma unroll
                 for (int e = 0; e < 16; ++e) atomicAdd(gp + (int64_t)e * (a.kh * a.kw), a.scale * __uint_as_float(rr[e]));
             }
         }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, BN);
     }
 }
 
@@ -501,8 +500,8 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
 //   grad_offset  = sum_c colg * mask * d bilinear / d position      (K10, :694-766)
 //   grad_mask    = sum_c colg * bilinear(x)                         (K10, :752)
 // One CTA owns one 8 x 16 pixel tile and a subset of the taps.  For a tap and a 128-channel chunk the 128 x 128 block of colg is one
-// tcgen05 GEMM over Cout (A = re-tiled grad_output, MN-major: pixels contiguous; B = the forward's packed weights read MN-major:
-// (tap, channel) contiguous; bf16 hi / lo, three MMAs per K block) into one of two TMEM accumulators.  The 16 epilogue warps move
+// wgmma GEMM over Cout (A = re-tiled grad_output, MN-major: pixels contiguous; B = the forward's packed weights read MN-major:
+// (tap, channel) contiguous; bf16 hi / lo, three MMAs per K block) into the MMA warpgroup's register accumulator, published as a shared-memory tile.  The 16 epilogue warps move
 // it through a swizzled fp32 staging tile to the forward's 8-lanes-per-pixel mapping, gather the four corners from the NHWC input
 // (128 contiguous bytes per 8 lanes), form the three per-pixel sums and scatter into an NHWC fp32 copy of grad_input with 16-byte
 // vector reductions (red.global.add.v4.f32), which a transpose-add folds into the caller's NCHW tensor.
@@ -524,7 +523,8 @@ struct DcnDSmem {
     static constexpr int STAGES = 2;                          // small on purpose: the epilogue's gathers want the rest of the SM's L1
     static constexpr int STG_OFF = STAGES * STAGE_BYTES;      // fp32 staging tile [128 pixels][128 channels], 16-byte chunks XOR-swizzled
     static constexpr int STG_BYTES = BM * BN * 4;
-    static constexpr int BAR_OFF = STG_OFF + STG_BYTES;
+    static constexpr int ACC_OFF = STG_OFF + STG_BYTES;       // the accumulator tile the MMA warpgroup publishes
+    static constexpr int BAR_OFF = ACC_OFF + (AccTile<BN>::BYTES + 127) / 128 * 128;
     static constexpr int TAB_OFF = BAR_OFF + 128;
     static constexpr int TAB_BYTES = 2 * BM * (3 * 16 + 8 + 4);          // tap tables, double-buffered by tap parity
     static constexpr int TOTAL = TAB_OFF + TAB_BYTES + 1024;
@@ -581,14 +581,13 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                          const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, DcnDArgs a) {
     using L = DcnDSmem;
     constexpr int STAGES = L::STAGES;
-    constexpr uint32_t BN = L::BN;
+    constexpr int BN = L::BN;
     extern __shared__ unsigned char smem_raw[];
     unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
     uint64_t *empty = full + STAGES;
     uint64_t *acc_full = empty + STAGES;
     uint64_t *acc_empty = acc_full + 2;
-    uint32_t *tmem_slot = (uint32_t *)(acc_empty + 2);
     auto tab_of = [&](int tb) {
         DcnDTab t;
         unsigned char *base = smem + L::TAB_OFF + tb * (L::TAB_BYTES / 2);
@@ -609,12 +608,51 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
         for (int s = 0; s < 2; ++s) { mbar_init(acc_full + s, 1); mbar_init(acc_empty + s, kProducerThreads / 32); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 2 * BN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    float *acc_tile = (float *)(smem + L::ACC_OFF);
 
+    // 768 threads leave 80 registers each: the MMA warpgroup takes what its 128 accumulator registers need from the others
+    if (threadIdx.x >= kDcnMma0) {
+        reg_inc<160>();
+        // both operands MN-major.  The accumulator of block n lives in registers, so its MMAs overlap the epilogue of block
+        // n - 1; only the publication into the single shared tile waits until the epilogue warps have drained that block.
+        const int mt = threadIdx.x - kDcnMma0;
+        AccTile<BN> acc;
+        int i = 0, n = 0;
+        for (int kk = blockIdx.y; kk < K; kk += a.tap_splits)
+            for (int h = 0; h < a.nch; ++h, ++n) {
+                const int buf = n & 1;
+                uint64_t *pending = nullptr;
+                for (int kb = 0; kb < a.nkk; ++kb, ++i) {
+                    const int s = i % STAGES;
+                    mbar_wait(full + s, (i / STAGES) & 1);
+                    const uint32_t ah = smem_u32(smem + s * L::STAGE_BYTES);
+                    const uint32_t al = ah + L::OP_BYTES, bh = ah + 2 * L::OP_BYTES, bl = ah + 3 * L::OP_BYTES;
+                    wgmma_fence();
+#pragma unroll
+                    for (int pass = 0; pass < 3; ++pass) {
+                        const uint32_t aa = pass == 2 ? al : ah, bb = pass == 1 ? bl : bh;
+#pragma unroll
+                        for (int k4 = 0; k4 < L::KB / UMMA_K; ++k4)
+                            acc.mma_halves<1, 1>(make_desc(aa + k4 * 2048, L::KB * 128, 1024), make_desc(aa + L::KB * 128 + k4 * 2048, L::KB * 128, 1024),
+                                                 make_desc(bb + k4 * 2048, L::KB * 128, 1024), make_desc(bb + L::KB * 128 + k4 * 2048, L::KB * 128, 1024),
+                                                 (kb | pass | k4) != 0);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    if (pending && mt == 0) mbar_arrive_cta(pending);
+                    pending = empty + s;
+                }
+                wgmma_wait<0>();
+                if (pending && mt == 0) mbar_arrive_cta(pending);
+                if (n > 0) mbar_wait(acc_empty + (buf ^ 1), ((n - 1) >> 1) & 1);
+                acc.store(acc_tile, mt);
+                mma_group_sync();
+                if (mt == 0) mbar_arrive_cta(acc_full + buf);
+            }
+        return;
+    }
+    reg_dec<64>();
     if (warp == 0) {
         if (elect_one()) {
             int i = 0;
@@ -637,37 +675,8 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                         tma_load_2d(&tmWl, full + s, st + 3 * L::OP_BYTES + L::KB * 128, kc1, kb * L::KB);
                     }
         }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = make_idesc(BM, BN, 1, 1);                             // both operands MN-major
-        int i = 0, n = 0;
-        for (int kk = blockIdx.y; kk < K; kk += a.tap_splits)
-            for (int h = 0; h < a.nch; ++h, ++n) {
-                const int buf = n & 1;
-                mbar_wait(acc_empty + buf, ((n >> 1) & 1) ^ 1);
-                tc_fence_after();
-                for (int kb = 0; kb < a.nkk; ++kb, ++i) {
-                    const int s = i % STAGES;
-                    mbar_wait(full + s, (i / STAGES) & 1);
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint32_t ah = smem_u32(smem + s * L::STAGE_BYTES);
-                        const uint32_t al = ah + L::OP_BYTES, bh = ah + 2 * L::OP_BYTES, bl = ah + 3 * L::OP_BYTES;
-#pragma unroll
-                        for (int pass = 0; pass < 3; ++pass) {
-                            const uint32_t aa = pass == 2 ? al : ah, bb = pass == 1 ? bl : bh;
-#pragma unroll
-                            for (int k4 = 0; k4 < L::KB / UMMA_K; ++k4)
-                                umma_bf16(tmem_base + buf * BN, make_desc(aa + k4 * 2048, L::KB * 128, 1024),
-                                          make_desc(bb + k4 * 2048, L::KB * 128, 1024), idesc, (kb | pass | k4) != 0);
-                        }
-                        umma_commit(empty + s);
-                        if (kb == a.nkk - 1) umma_commit(acc_full + buf);
-                    }
-                    __syncwarp();
-                }
-            }
-    } else {
-        // Epilogue warp = (TMEM quarter q, slice `part`).  It drains 32 channels of its quarter's 32 pixel rows into the shared staging tile
+    } else if (warp >= 2 && threadIdx.x < 64 + kProducerThreads) {
+        // Epilogue warp = (row quarter q, slice `part`).  It drains 32 channels of its quarter's 32 pixel rows into the shared staging tile
         // and then owns 8 of those rows for all 128 channels (8 lanes per row, 2 rows per lane: the forward's gather mapping), so the sums
         // over channels stay in registers.  Only the four warps of a quarter synchronise (named barriers 1 + q and 5 + q); the quarters
         // drift apart, which overlaps one quarter's gather latency with another's arithmetic.
@@ -691,10 +700,9 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
             for (int h = 0; h < a.nch; ++h, ++n) {
                 const int buf = n & 1;
                 mbar_wait(acc_full + buf, (n >> 1) & 1);
-                tc_fence_after();
                 {
                     uint32_t rr[32];
-                    tmem_ld32(tmem_base + buf * BN + ((uint32_t)(q * 32) << 16) + (uint32_t)(part * 32), rr);
+                    acc_ld<32>(acc_tile, AccTile<BN>::LD, q * 32, part * 32, rr);
                     const int r = R0 + lane;
                     const uint32_t rb = stg + (uint32_t)r * 512u;
 #pragma unroll
@@ -702,7 +710,6 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                         asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(rb + ((((uint32_t)(part * 8 + c4)) ^ (uint32_t)(r & 31)) << 4)),
                                      "r"(rr[4 * c4]), "r"(rr[4 * c4 + 1]), "r"(rr[4 * c4 + 2]), "r"(rr[4 * c4 + 3]) : "memory");
                 }
-                tc_fence_before();
                 asm volatile("bar.sync %0, 128;" ::"r"(1 + q) : "memory");
                 if (lane == 0) mbar_arrive_cta(acc_empty + buf);
                 // the next tap's table: its three global loads are issued now and consumed after this N block's work
@@ -778,12 +785,6 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                 }
             }
         }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 2 * BN);
     }
 }
 
@@ -962,20 +963,17 @@ int mr_dcn_forward_fused_f32(const float *input, const float *weight, const floa
     int rc = check_launch("dcn_nchw_to_nhwc_kernel");
     if (rc) return rc;
     const int64_t nw = (int64_t)Cout * C * kh * kw;
-    dcn_weight_pack_kernel<<<(unsigned)std::min<int64_t>(ceil_div(nw, 256), 148 * 8), 256, 0, st>>>(weight, Cout, C, kh * kw, whi, wlo);
+    dcn_weight_pack_kernel<<<(unsigned)std::min<int64_t>(ceil_div(nw, 256), sm_count() * 8), 256, 0, st>>>(weight, Cout, C, kh * kw, whi, wlo);
     rc = check_launch("dcn_weight_pack_kernel");
     if (rc) return rc;
     a.xh = xh; a.off = offset; a.msk = mask; a.bias = bias; a.out = output; a.off_bs = offset_bstride; a.mask_bs = mask_bstride;
     const int64_t Kt = (int64_t)kh * kw * C;
-    /* BN = 256 halves the number of times a pixel tile is gathered when Cout >= 256, as long as the grid still covers the SMs */
-    const bool wide = Cout % 256 == 0 && (int64_t)B * a.tiles_per_sample * (Cout / 256) >= sm_count();
     CUtensorMap th, tl;
-    rc = make_map(&th, whi, Kt, Cout, Kt, BK, wide ? 256 : 128);
+    rc = make_map(&th, whi, Kt, Cout, Kt, BK, 128);
     if (rc) return rc;
-    rc = make_map(&tl, wlo, Kt, Cout, Kt, BK, wide ? 256 : 128);
+    rc = make_map(&tl, wlo, Kt, Cout, Kt, BK, 128);
     if (rc) return rc;
-    if (wide) return launch_dcn_fwd<256, 2>(th, tl, a, st);
-    /* two stages, not three: the 64 KB saved become L1 for the gathers (measured 83 -> 76 us at C = 128 @ 64 x 64, B = 8) */
+    /* two stages, not three: the 64 KB saved become L1 for the gathers (MR_DCN_STAGES3 selects three for experiments) */
     static const bool three = getenv("MR_DCN_STAGES3") != nullptr;
     if (three) return launch_dcn_fwd<128, 3>(th, tl, a, st);
     return launch_dcn_fwd<128, 2>(th, tl, a, st);
@@ -1034,7 +1032,7 @@ int mr_dcn_backward_fused_f32(const float *input, const float *weight, const flo
     }
     if (want_data) {
         const int64_t nw = (int64_t)Cout * C * kh * kw;
-        dcn_weight_pack_kernel<<<(unsigned)std::min<int64_t>(ceil_div(nw, 256), 148 * 8), 256, 0, st>>>(weight, Cout, C, kh * kw, whi, wlo);
+        dcn_weight_pack_kernel<<<(unsigned)std::min<int64_t>(ceil_div(nw, 256), sm_count() * 8), 256, 0, st>>>(weight, Cout, C, kh * kw, whi, wlo);
         rc = check_launch("dcn_weight_pack_kernel");
         if (rc) return rc;
         if (grad_input) MR_CUDA_TRY(cudaMemsetAsync(gxh, 0, (size_t)B * H * W * C * 4, st), "cudaMemsetAsync(dcn grad_input scratch)");

@@ -1,4 +1,4 @@
-// Deformable position-sensitive RoI pooling for sm_100a (SURVEY.md section 8 rows A13 / N4): replaces
+// Deformable position-sensitive RoI pooling for sm_90a (SURVEY.md section 8 rows A13 / N4): replaces
 // assets/ops/dcn/src/deform_pool_cuda_kernel.cu:52-263 + deform_pool_cuda.cpp:29-81 behind the same five-plus-arguments
 // surface (functions/deform_pool.py:7-69).  fp32.
 //
@@ -159,7 +159,7 @@ int mr_deform_psroi_pool_forward_f32(const float *data, const float *rois, const
     if (num_rois == 0) return MR_OK;
     if (!data || !rois || !out || !top_count || (!no_trans && !trans)) return MR_ERR_NULL_POINTER;
     const int64_t count = (int64_t)num_rois * output_dim * pooled_size * pooled_size;
-    const int blocks = (int)((count + 255) / 256 < 148 * 16 ? (count + 255) / 256 : 148 * 16);
+    const int blocks = (int)((count + 255) / 256 < mr::sm_count() * 16 ? (count + 255) / 256 : mr::sm_count() * 16);
     deform_psroi_fwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a, count, data, rois, trans, out, top_count);
     return check_launch("deform_psroi_fwd_kernel");
 }
@@ -178,7 +178,7 @@ int mr_deform_psroi_pool_backward_f32(const float *out_grad, const float *data, 
     if (num_rois == 0) return MR_OK;
     if (!out_grad || !data || !rois || !top_count || !in_grad || (!no_trans && (!trans || !trans_grad))) return MR_ERR_NULL_POINTER;
     const int64_t count = (int64_t)num_rois * output_dim * pooled_size * pooled_size;
-    const int blocks = (int)((count + 255) / 256 < 148 * 16 ? (count + 255) / 256 : 148 * 16);
+    const int blocks = (int)((count + 255) / 256 < mr::sm_count() * 16 ? (count + 255) / 256 : mr::sm_count() * 16);
     deform_psroi_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a, count, out_grad, top_count, data, rois, trans, in_grad, trans_grad);
     return check_launch("deform_psroi_bwd_kernel");
 }

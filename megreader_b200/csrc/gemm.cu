@@ -1,6 +1,6 @@
 // Plain dense GEMMs of the engine: row-major  C[M,N] = alpha * op(A) * op(B) + beta * C  with fp32 accumulation.
 // This revision routes them to cuBLAS (cublasGemmEx / cublasGemmStridedBatchedEx) — "plain library GEMMs" per the
-// build rules; the conv / LSTM *fusions* around them are this repo's kernels.  A tcgen05 + TMA kernel replaces the
+// build rules; the conv / LSTM *fusions* around them are this repo's kernels.  A wgmma + TMA kernel replaces the
 // dominant shapes behind the same entry point (csrc/gemm_tcgen05.cu) when MR_GEMM_BACKEND selects it.
 //
 // Row-major <-> cuBLAS column-major: C^T = op(B)^T op(A)^T, so the operands are swapped and an operand that is

@@ -1,5 +1,6 @@
-// Blackwell-native dense GEMM: bf16 operands, fp32 accumulation in TMEM (tcgen05.mma, cta_group::1, UMMA 128xBNx16),
-// operands staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) through a 4..6-stage mbarrier ring.
+// Hopper dense GEMM: bf16 operands, fp32 accumulation in the registers of one MMA warpgroup (wgmma.mma_async m64nBNk16,
+// two per K step for the 128-row tile), operands staged by TMA (cp.async.bulk.tensor, 128-byte swizzle) through a
+// 3..8-stage mbarrier ring.
 //
 //   C[M,N] (row-major, bf16 or fp32)  (+)=  op(A)[M,K] * op(B)[K,N]
 //     A_MN = 0: A stored [M,K] row-major (K-major operand)        A_MN = 1: A stored [K,M] row-major (MN-major operand)
@@ -8,10 +9,11 @@
 //   gradients  dW[Cout, K] = dZ[P, Cout]^T * col[P, K].
 //   Epilogue: optional per-column bias, optional ReLU, fp32 or bf16 store, or fp32 atomic accumulation (split-K).
 //
-// Warp roles (192 threads): warp 0 = TMA producer (one elected lane), warp 1 = TMEM allocator + MMA issuer (one
-// elected lane), warps 2..5 = epilogue (TMEM -> registers -> global), each owning the 32 TMEM lanes its warp id
-// (mod 4) may touch.  One 128 x BN output tile per CTA (grid = tiles x split-K); K loops over 64-element blocks.
-#include "tcgen05.cuh"
+// Warp roles (384 threads): warp 0 = TMA producer (one elected lane), warps 2..5 = epilogue (one accumulator row per
+// thread -> global), warps 8..11 = the MMA warpgroup, which hands the finished accumulator to the epilogue warps through
+// a shared-memory tile laid over the drained operand ring.  One 128 x BN output tile (BN <= 128: the accumulator is
+// BN registers per MMA thread) per CTA (grid = tiles x split-K); K loops over 64-element blocks.
+#include "wgmma.cuh"
 #include <stdlib.h>
 
 namespace {
@@ -25,24 +27,23 @@ struct GemmArgs {
     int kblocks_per_split;
 };
 
-// Epilogue shared by the GEMM and convolution kernels: warps 2..5, TMEM -> registers -> (bias, ReLU) -> global.
+// Epilogue shared by the GEMM and convolution kernels: warps 2..5, accumulator tile -> registers -> (bias, ReLU) -> global.
 template <int BN>
-__device__ __forceinline__ void epilogue_store(const GemmArgs &g, uint32_t tmem_base, uint64_t *tmem_full, int m0, int n0,
+__device__ __forceinline__ void epilogue_store(const GemmArgs &g, const float *acc, uint64_t *tmem_full, int m0, int n0,
                                                int warp, int lane, bool have_acc, int64_t row_override = -2) {
-        const int q = warp & 3;                               // TMEM lane quarter this warp may access
+        const int q = warp & 3;                               // 32-row quarter of the tile this warp stores
         // output row of this thread: m0 + tile row, or an explicit row (-1 = none) for tiles that are not row ranges
         const int64_t row = row_override == -2 ? (int64_t)(m0 + q * 32 + lane) : (row_override < 0 ? (int64_t)g.M : row_override);
         const int nkb = have_acc ? 1 : 0;
         if (nkb > 0) {
             mbar_wait(tmem_full, 0);
-            tc_fence_after();
         }
         float *Cf = (float *)g.C;
         bf16 *Ch = (bf16 *)g.C;
 #pragma unroll 1
         for (int c = 0; c < BN / 32; ++c) {
             uint32_t r[32];
-            if (nkb > 0) tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(c * 32), r);
+            if (nkb > 0) acc_ld<32>(acc, AccTile<BN>::LD, q * 32, c * 32, r);
             else {
 #pragma unroll
                 for (int j = 0; j < 32; ++j) r[j] = 0;
@@ -93,6 +94,36 @@ __device__ __forceinline__ void epilogue_store(const GemmArgs &g, uint32_t tmem_
         }
 }
 
+constexpr int kGemmMma0 = 256;                      // first thread of the MMA warpgroup (warps 6, 7 are padding)
+constexpr int kGemmThreads = kGemmMma0 + kMmaThreads;
+
+// The MMA warpgroup's K loop over the ring: wgmma for stage i is committed, then stage i - 1 is known to have retired and
+// its slot is handed back to the producers.  issue(i, s) queues the wgmmas of one stage.
+template <typename Issue>
+__device__ __forceinline__ void mma_ring(int nkb, int stages, uint64_t *full, uint64_t *empty, bool leader, Issue issue) {
+    uint64_t *pending = nullptr;
+    for (int i = 0; i < nkb; ++i) {
+        const int s = i % stages;
+        mbar_wait(full + s, (i / stages) & 1);
+        wgmma_fence();
+        issue(i, s);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (pending && leader) mbar_arrive(pending);
+        pending = empty + s;
+    }
+    wgmma_wait<0>();
+    if (pending && leader) mbar_arrive(pending);
+}
+// ... and the hand-over: the ring is drained (every load was consumed), so the accumulator tile is laid over it.
+template <int BN>
+__device__ __forceinline__ void mma_publish(const AccTile<BN> &acc, float *tile, uint64_t *tmem_full, int mt) {
+    mma_group_sync();
+    acc.store(tile, mt);
+    mma_group_sync();
+    if (mt == 0) mbar_arrive(tmem_full);
+}
+
 template <int BN, int STAGES>
 struct SmemLayout {
     static constexpr int A_BYTES = BM * BK * 2;      // 16 KB
@@ -100,10 +131,11 @@ struct SmemLayout {
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
     static constexpr int TOTAL = BAR_OFF + (2 * STAGES + 1) * 8 + 16 + 1024;   // + alignment slack
+    static_assert(AccTile<BN>::BYTES <= BAR_OFF, "the accumulator tile is laid over the operand ring");
 };
 
 template <int BN, int STAGES, int A_MN, int B_MN>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmArgs g) {
     using L = SmemLayout<BN, STAGES>;
     extern __shared__ unsigned char smem_raw[];
@@ -111,7 +143,6 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
     uint64_t *empty = full + STAGES;
     uint64_t *tmem_full = empty + STAGES;
-    uint32_t *tmem_slot = (uint32_t *)(tmem_full + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
@@ -119,7 +150,6 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     const int kb_lo = blockIdx.z * g.kblocks_per_split;
     const int kb_hi = min(kb_total, kb_lo + g.kblocks_per_split);
     const int nkb = kb_hi - kb_lo;
-    constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmA);
@@ -128,11 +158,8 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         mbar_init(tmem_full, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    float *acc_tile = (float *)smem;
 
     if (warp == 0) {
         // ------------------------------------------------------------ TMA producer
@@ -157,42 +184,30 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
                 }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------ MMA issuer
-        constexpr uint32_t idesc = make_idesc(BM, BN, A_MN, B_MN);
-        for (int i = 0; i < nkb; ++i) {
-            const int s = i % STAGES;
-            const uint32_t ph = (i / STAGES) & 1;
-            mbar_wait(full + s, ph);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
-                const uint32_t b_addr = a_addr + L::A_BYTES;
+    } else if (threadIdx.x >= kGemmMma0) {
+        // ------------------------------------------------------------ MMA warpgroup
+        const int mt = threadIdx.x - kGemmMma0;
+        AccTile<BN> acc;
+        mma_ring(nkb, STAGES, full, empty, mt == 0, [&](int i, int s) {
+            const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
+            const uint32_t b_addr = a_addr + L::A_BYTES;
 #pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k) {
-                    // K-major: 8-row groups 1024 B apart (SBO), advance 32 B per UMMA_K inside the 128 B atom.
-                    // MN-major: 64-element M/N atoms BK*128 B apart (LBO), 8-row K groups 1024 B apart (SBO),
-                    //           advance 16 rows * 128 B per UMMA_K.
-                    const uint64_t ad = A_MN == 0 ? make_desc(a_addr + k * 32, 16, 1024)
-                                                  : make_desc(a_addr + k * 2048, BK * 128, 1024);
-                    const uint64_t bd = B_MN == 0 ? make_desc(b_addr + k * 32, 16, 1024)
-                                                  : make_desc(b_addr + k * 2048, BK * 128, 1024);
-                    umma_bf16(tmem_base, ad, bd, idesc, (i | k) != 0);
-                }
-                umma_commit(empty + s);                       // frees the smem slot when these MMAs retire
-                if (i == nkb - 1) umma_commit(tmem_full);     // accumulator complete
+            for (int k = 0; k < BK / UMMA_K; ++k) {
+                // K-major: 8-row groups 1024 B apart (SBO), advance 32 B per 16-deep step inside the 128 B atom; the
+                //          tile's lower 64 rows start 64 * 128 B further on.
+                // MN-major: 64-element M/N atoms BK*128 B apart (LBO), 8-row K groups 1024 B apart (SBO),
+                //           advance 16 rows * 128 B per step; the lower 64 rows are the second atom.
+                const uint64_t a_lo = A_MN == 0 ? make_desc(a_addr + k * 32, 16, 1024) : make_desc(a_addr + k * 2048, BK * 128, 1024);
+                const uint64_t a_hi = A_MN == 0 ? make_desc(a_addr + 64 * 128 + k * 32, 16, 1024)
+                                                : make_desc(a_addr + BK * 128 + k * 2048, BK * 128, 1024);
+                const uint64_t bd = B_MN == 0 ? make_desc(b_addr + k * 32, 16, 1024) : make_desc(b_addr + k * 2048, BK * 128, 1024);
+                acc.template mma<A_MN, B_MN>(a_lo, a_hi, bd, (i | k) != 0);
             }
-            __syncwarp();
-        }
-    } else {
+        });
+        if (nkb > 0) mma_publish<BN>(acc, acc_tile, tmem_full, mt);
+    } else if (warp >= 2 && threadIdx.x < 192) {
         // ------------------------------------------------------------ epilogue (warps 2..5)
-        epilogue_store<BN>(g, tmem_base, tmem_full, m0, n0, warp, lane, nkb > 0);
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
+        epilogue_store<BN>(g, acc_tile, tmem_full, m0, n0, warp, lane, nkb > 0);
     }
 }
 
@@ -203,7 +218,7 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
 //
 // The im2col matrix never exists in HBM: warps 2..5 (one thread per output pixel of the 128-row tile) gather the
 // 128-byte channel chunk of each row with zero-filling cp.async straight into the 128B-swizzled K-major smem tile
-// that tcgen05.mma reads (chunk j of row r lands at r*128 + ((j ^ (r & 7)) << 4)); the weight tile comes by TMA.
+// that wgmma.mma_async reads (chunk j of row r lands at r*128 + ((j ^ (r & 7)) << 4)); the weight tile comes by TMA.
 // The same kernel computes the input gradient: dgrad of a stride-1 convolution is a convolution of dz with the
 // flipped / transposed weights and padding (k-1-p).  Requires C % 64 == 0.
 // =====================================================================================================
@@ -214,7 +229,7 @@ struct ConvArgs {
     // TMA-A variant: the output space [N, Ho, Wo] is tiled by boxes of bw x bh x bn = 128 pixels; the width is cut
     // into segments of power-of-two widths (e.g. Wo = 65 -> one 64-wide segment + one 1-wide segment).
     struct Seg { int w0, bw, bh, bn, h_blocks, tile_begin; } seg[4];
-    int nseg, ntiles;
+    int nseg;
     GemmArgs g;        // M = N*Ho*Wo, N = Cout, K = kh*kw*C
 };
 
@@ -225,16 +240,12 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap *map, uint64_t *ba
 __device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void *src, uint32_t src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
 
-// MT = number of 128-row sub-tiles per CTA (1 or 2).  MT = 2 shares every weight tile between two activation
-// sub-tiles (two TMEM accumulators): operand bytes per FLOP drop by a third, which matters because the first
-// version of this kernel was bound by L2 -> SM operand traffic (10 TB/s, profiles/conv_fprop_r1a_summary.md).
-template <int BN, int STAGES, int MT>
+// One 128-row tile per CTA: a second accumulator would double the MMA warpgroup's register need (BN registers per thread
+// per tile), which is a limit of the one-warpgroup design, not a measured choice.
+template <int BN, int STAGES>
 struct ConvSmem {
-    static constexpr int A_BYTES = MT * BM * BK * 2;
+    static constexpr int A_BYTES = BM * BK * 2;
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
@@ -243,25 +254,24 @@ struct ConvSmem {
 
 // TMA_A = 1: "same"-padded convolutions whose 128-pixel tiles are whole row segments (W | 128 or 128 | W) fetch the
 // activation tile with ONE 4-D TMA per K block (tap shift = signed coordinate offset, padding = TMA zero fill)
-// instead of 1024 cp.async from the LSU, which capped the gather at one tile per ~256 cycles.
-template <int BN, int STAGES, int MT, int TMA_A>
-__global__ void __launch_bounds__(192, 1)
+// instead of 1024 cp.async from the LSU.
+template <int BN, int STAGES, int TMA_A>
+__global__ void __launch_bounds__(kGemmThreads, 1)
 conv_fprop_tcgen05_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmX0,
                           const __grid_constant__ CUtensorMap tmX1, const __grid_constant__ CUtensorMap tmX2,
                           const __grid_constant__ CUtensorMap tmX3, ConvArgs a) {
-    using L = ConvSmem<BN, STAGES, MT>;
+    using L = ConvSmem<BN, STAGES>;
+    static_assert(AccTile<BN>::BYTES <= L::BAR_OFF, "the accumulator tile is laid over the operand ring");
     extern __shared__ unsigned char smem_raw[];
     unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
     uint64_t *empty = full + STAGES;
     uint64_t *tmem_full = empty + STAGES;
-    uint32_t *tmem_slot = (uint32_t *)(tmem_full + 1);
     const GemmArgs &g = a.g;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int m0 = blockIdx.x * (BM * MT), n0 = blockIdx.y * BN;
+    const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
     const int cchunks = a.C / BK;
     const int nkb = a.kh * a.kw * cchunks;
-    constexpr uint32_t TMEM_COLS = (MT * BN) < 32 ? 32 : (MT * BN);
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmB);
@@ -270,34 +280,24 @@ conv_fprop_tcgen05_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_
         mbar_init(tmem_full, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    float *acc_tile = (float *)smem;
 
     if (warp == 0) {
         if (elect_one()) {                                   // weight tiles (and, with TMA_A, activation tiles) by TMA
-            // TMA_A: this CTA owns MT consecutive tiles of the segment enumeration (tile id = blockIdx.x * MT + sub); a
-            // tile id past the end (odd tile count) loads an all-out-of-bounds box (zero fill) and stores nothing
-            int tn[MT], th0[MT], tw0[MT];
-            const CUtensorMap *tmX[MT];
-#pragma unroll
-            for (int sub = 0; sub < MT; ++sub) {
-                tn[sub] = th0[sub] = tw0[sub] = 0;
-                tmX[sub] = &tmX0;
-                if (TMA_A) {
-                    const int tile = (int)blockIdx.x * MT + sub;
-                    if (tile >= a.ntiles) { tn[sub] = a.N; continue; }
-                    int sel = 0;
-                    for (int q = 1; q < a.nseg; ++q) if (tile >= a.seg[q].tile_begin) sel = q;
-                    const int lt = tile - a.seg[sel].tile_begin;
-                    const int nb = lt / a.seg[sel].h_blocks;
-                    tn[sub] = nb * a.seg[sel].bn;
-                    th0[sub] = (lt - nb * a.seg[sel].h_blocks) * a.seg[sel].bh;
-                    tw0[sub] = a.seg[sel].w0;
-                    tmX[sub] = sel == 0 ? &tmX0 : (sel == 1 ? &tmX1 : (sel == 2 ? &tmX2 : &tmX3));
-                }
+            // TMA_A: this CTA owns tile blockIdx.x of the segment enumeration
+            int tn = 0, th0 = 0, tw0 = 0;
+            const CUtensorMap *tmX = &tmX0;
+            if (TMA_A) {
+                const int tile = (int)blockIdx.x;
+                int sel = 0;
+                for (int q = 1; q < a.nseg; ++q) if (tile >= a.seg[q].tile_begin) sel = q;
+                const int lt = tile - a.seg[sel].tile_begin;
+                const int nb = lt / a.seg[sel].h_blocks;
+                tn = nb * a.seg[sel].bn;
+                th0 = (lt - nb * a.seg[sel].h_blocks) * a.seg[sel].bh;
+                tw0 = a.seg[sel].w0;
+                tmX = sel == 0 ? &tmX0 : (sel == 1 ? &tmX1 : (sel == 2 ? &tmX2 : &tmX3));
             }
             int cc = 0, ti = 0, tj = 0;
             for (int i = 0; i < nkb; ++i) {
@@ -305,71 +305,52 @@ conv_fprop_tcgen05_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_
                 mbar_wait(empty + s, ((i / STAGES) & 1) ^ 1);
                 mbar_expect_tx(full + s, TMA_A ? L::STAGE_BYTES : L::B_BYTES);
                 if (TMA_A) {
-#pragma unroll
-                    for (int sub = 0; sub < MT; ++sub)
-                        tma_load_4d(tmX[sub], full + s, smem + s * L::STAGE_BYTES + sub * (BM * BK * 2), cc * BK,
-                                    tw0[sub] * a.sw + tj * a.dw - a.pw, th0[sub] * a.sh + ti * a.dh - a.ph, tn[sub]);
+                    tma_load_4d(tmX, full + s, smem + s * L::STAGE_BYTES, cc * BK, tw0 * a.sw + tj * a.dw - a.pw,
+                                th0 * a.sh + ti * a.dh - a.ph, tn);
                     if (++cc == cchunks) { cc = 0; if (++tj == a.kw) { tj = 0; ++ti; } }
                 }
                 tma_load_2d(&tmB, full + s, smem + s * L::STAGE_BYTES + L::A_BYTES, i * BK, n0);
             }
         }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = make_idesc(BM, BN, 0, 0);
-        for (int i = 0; i < nkb; ++i) {
-            const int s = i % STAGES;
-            mbar_wait(full + s, (i / STAGES) & 1);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
-                const uint32_t b_addr = a_addr + L::A_BYTES;
+    } else if (threadIdx.x >= kGemmMma0) {
+        // ------------------------------------------------------------ MMA warpgroup
+        const int mt = threadIdx.x - kGemmMma0;
+        AccTile<BN> acc;
+        mma_ring(nkb, STAGES, full, empty, mt == 0, [&](int i, int s) {
+            const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
+            const uint32_t b_addr = a_addr + L::A_BYTES;
 #pragma unroll
-                for (int sub = 0; sub < MT; ++sub) {
-#pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k)
-                        umma_bf16(tmem_base + sub * BN, make_desc(a_addr + sub * (BM * BK * 2) + k * 32, 16, 1024),
-                                  make_desc(b_addr + k * 32, 16, 1024), idesc, (i | k) != 0);
-                }
-                umma_commit(empty + s);
-                if (i == nkb - 1) umma_commit(tmem_full);
-            }
-            __syncwarp();
-        }
+            for (int k = 0; k < BK / UMMA_K; ++k)
+                acc.template mma<0, 0>(make_desc(a_addr + k * 32, 16, 1024), make_desc(a_addr + 64 * 128 + k * 32, 16, 1024),
+                                       make_desc(b_addr + k * 32, 16, 1024), (i | k) != 0);
+        });
+        if (nkb > 0) mma_publish<BN>(acc, acc_tile, tmem_full, mt);
+    } else if (warp < 2 || threadIdx.x >= 192) {
+        // warp 1 and the padding warps have no role
     } else if (TMA_A) {
-#pragma unroll
-        for (int sub = 0; sub < MT; ++sub) {
-            const int tile = (int)blockIdx.x * MT + sub;
-            int64_t prow = -1;
-            if (tile < a.ntiles) {
-                int sel = 0;
-                for (int q = 1; q < a.nseg; ++q) if (tile >= a.seg[q].tile_begin) sel = q;
-                const int lt = tile - a.seg[sel].tile_begin;
-                const int nb = lt / a.seg[sel].h_blocks;
-                const int bw = a.seg[sel].bw, bh = a.seg[sel].bh;
-                const int r = (warp & 3) * 32 + lane;        // tile row = (dn * bh + dh) * bw + dw
-                const int dw = r % bw, dh = (r / bw) % bh, dn = r / (bw * bh);
-                const int pn = nb * a.seg[sel].bn + dn, phh = (lt - nb * a.seg[sel].h_blocks) * bh + dh, pww = a.seg[sel].w0 + dw;
-                if (pn < a.N && phh < a.Ho && pww < a.Wo) prow = ((int64_t)pn * a.Ho + phh) * a.Wo + pww;
-            }
-            epilogue_store<BN>(g, tmem_base + sub * BN, tmem_full, 0, n0, warp, lane, nkb > 0, prow);
-        }
-        tc_fence_before();
+        const int tile = (int)blockIdx.x;
+        int64_t prow = -1;
+        int sel = 0;
+        for (int q = 1; q < a.nseg; ++q) if (tile >= a.seg[q].tile_begin) sel = q;
+        const int lt = tile - a.seg[sel].tile_begin;
+        const int nb = lt / a.seg[sel].h_blocks;
+        const int bw = a.seg[sel].bw, bh = a.seg[sel].bh;
+        const int r = (warp & 3) * 32 + lane;                // tile row = (dn * bh + dh) * bw + dw
+        const int dw = r % bw, dh = (r / bw) % bh, dn = r / (bw * bh);
+        const int pn = nb * a.seg[sel].bn + dn, phh = (lt - nb * a.seg[sel].h_blocks) * bh + dh, pww = a.seg[sel].w0 + dw;
+        if (pn < a.N && phh < a.Ho && pww < a.Wo) prow = ((int64_t)pn * a.Ho + phh) * a.Wo + pww;
+        epilogue_store<BN>(g, acc_tile, tmem_full, 0, n0, warp, lane, nkb > 0, prow);
     } else {
-        // ------------------------------------------------------------ activation gather (one thread = MT tile rows)
+        // ------------------------------------------------------------ activation gather (one thread = one tile row)
         const int r = threadIdx.x - 64;
-        bool valid[MT];
-        int n[MT], ho[MT], wo[MT];
-#pragma unroll
-        for (int sub = 0; sub < MT; ++sub) {
-            const int64_t p = (int64_t)m0 + sub * BM + r;
-            valid[sub] = p < g.M;
-            n[sub] = ho[sub] = wo[sub] = 0;
-            if (valid[sub]) {
-                wo[sub] = (int)(p % a.Wo);
-                const int64_t t = p / a.Wo;
-                ho[sub] = (int)(t % a.Ho);
-                n[sub] = (int)(t / a.Ho);
-            }
+        const int64_t p = (int64_t)m0 + r;
+        const bool valid = p < g.M;
+        int n = 0, ho = 0, wo = 0;
+        if (valid) {
+            wo = (int)(p % a.Wo);
+            const int64_t t = p / a.Wo;
+            ho = (int)(t % a.Ho);
+            n = (int)(t / a.Ho);
         }
         const uint32_t row_off = (uint32_t)r * 128u;
         const uint32_t sw = (uint32_t)(r & 7);
@@ -379,20 +360,17 @@ conv_fprop_tcgen05_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_
         for (int i = 0; i < nkb; ++i) {
             const int s = i % STAGES;
             mbar_wait(empty + s, ((i / STAGES) & 1) ^ 1);
+            const int h = ho * a.sh + ti * a.dh - a.ph, w = wo * a.sw + tj * a.dw - a.pw;
+            const bool ok = valid && h >= 0 && h < a.H && w >= 0 && w < a.W;
+            const bf16 *src = ok ? a.x + ((((int64_t)n * a.H + h) * a.W + w) * a.C + cc * BK) : a.x;
+            const uint32_t dst = smem_u32(smem + s * L::STAGE_BYTES) + row_off;
+            const uint32_t nbytes = ok ? 16u : 0u;
 #pragma unroll
-            for (int sub = 0; sub < MT; ++sub) {
-                const int h = ho[sub] * a.sh + ti * a.dh - a.ph, w = wo[sub] * a.sw + tj * a.dw - a.pw;
-                const bool ok = valid[sub] && h >= 0 && h < a.H && w >= 0 && w < a.W;
-                const bf16 *src = ok ? a.x + ((((int64_t)n[sub] * a.H + h) * a.W + w) * a.C + cc * BK) : a.x;
-                const uint32_t dst = smem_u32(smem + s * L::STAGE_BYTES + sub * (BM * BK * 2)) + row_off;
-                const uint32_t nbytes = ok ? 16u : 0u;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) cp_async16_zfill(dst + (((uint32_t)j ^ sw) << 4), src + j * 8, nbytes);
-            }
+            for (int j = 0; j < 8; ++j) cp_async16_zfill(dst + (((uint32_t)j ^ sw) << 4), src + j * 8, nbytes);
             cp_async_commit();
             if (i >= D - 1) {
                 cp_async_wait<D - 1>();
-                fence_proxy_async();                          // generic-proxy smem writes -> visible to tcgen05
+                fence_proxy_async();                          // generic-proxy smem writes -> visible to wgmma
                 mbar_arrive(full + (i - (D - 1)) % STAGES);
             }
             if (++cc == cchunks) { cc = 0; if (++tj == a.kw) { tj = 0; ++ti; } }
@@ -400,15 +378,7 @@ conv_fprop_tcgen05_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_
         cp_async_wait<0>();
         fence_proxy_async();
         for (int i = (nkb >= D - 1 ? nkb - (D - 1) : 0); i < nkb; ++i) mbar_arrive(full + i % STAGES);
-#pragma unroll
-        for (int sub = 0; sub < MT; ++sub)
-            epilogue_store<BN>(g, tmem_base + sub * BN, tmem_full, m0 + sub * BM, n0, warp, lane, nkb > 0);
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
+        epilogue_store<BN>(g, acc_tile, tmem_full, m0, n0, warp, lane, nkb > 0);
     }
 }
 
@@ -437,22 +407,21 @@ struct WgradSmem {
 };
 
 template <int BN, int RB, int STAGES>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
 conv_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant__ CUtensorMap tmX, WgradArgs a) {
     using L = WgradSmem<BN, RB, STAGES>;
+    static_assert(AccTile<BN>::BYTES <= L::BAR_OFF, "the accumulator tile is laid over the operand ring");
     extern __shared__ unsigned char smem_raw[];
     unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
     uint64_t *empty = full + STAGES;
     uint64_t *tmem_full = empty + STAGES;
-    uint32_t *tmem_slot = (uint32_t *)(tmem_full + 1);
     const GemmArgs &g = a.g;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
     const int kb_lo = blockIdx.z * a.kblocks_per_split;
     const int kb_hi = min(a.kb_total, kb_lo + a.kblocks_per_split);
     const int nkb = kb_hi - kb_lo;
-    constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmDz);
@@ -461,11 +430,8 @@ conv_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid
         mbar_init(tmem_full, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    float *acc_tile = (float *)smem;
 
     if (warp == 0) {
         if (elect_one()) {
@@ -501,39 +467,28 @@ conv_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid
                 }
             }
         }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = make_idesc(BM, BN, 1, 1);
-        for (int i = 0; i < nkb; ++i) {
-            const int s = i % STAGES;
-            mbar_wait(full + s, (i / STAGES) & 1);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
-                const uint32_t b_addr = a_addr + L::A_BYTES;
+    } else if (threadIdx.x >= kGemmMma0) {
+        // ------------------------------------------------------------ MMA warpgroup
+        const int mt = threadIdx.x - kGemmMma0;
+        AccTile<BN> acc;
+        mma_ring(nkb, STAGES, full, empty, mt == 0, [&](int i, int s) {
+            const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
+            const uint32_t b_addr = a_addr + L::A_BYTES;
 #pragma unroll
-                for (int k = 0; k < RB / UMMA_K; ++k)
-                    umma_bf16(tmem_base, make_desc(a_addr + k * 2048, RB * 128, 1024), make_desc(b_addr + k * 2048, RB * 128, 1024),
-                              idesc, (i | k) != 0);
-                umma_commit(empty + s);
-                if (i == nkb - 1) umma_commit(tmem_full);
-            }
-            __syncwarp();
-        }
-    } else {
-        epilogue_store<BN>(g, tmem_base, tmem_full, m0, n0, warp, lane, nkb > 0);
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
+            for (int k = 0; k < RB / UMMA_K; ++k)
+                acc.template mma<1, 1>(make_desc(a_addr + k * 2048, RB * 128, 1024), make_desc(a_addr + RB * 128 + k * 2048, RB * 128, 1024),
+                                       make_desc(b_addr + k * 2048, RB * 128, 1024), (i | k) != 0);
+        });
+        if (nkb > 0) mma_publish<BN>(acc, acc_tile, tmem_full, mt);
+    } else if (warp >= 2 && threadIdx.x < 192) {
+        epilogue_store<BN>(g, acc_tile, tmem_full, m0, n0, warp, lane, nkb > 0);
     }
 }
 
 // =====================================================================================================
 // Fused LSTM time step (decoders/crnn.py:13,17 nn.LSTM): recurrent GEMM + cell in ONE launch for both directions.
 // Gate columns are stored UNIT-MAJOR (column 4*j + g holds gate g of hidden unit j; g = i,f,g,o) so that the 32
-// accumulator columns a thread pulls from TMEM are 8 complete units.
+// accumulator columns a thread reads from the accumulator tile are 8 complete units.
 //   forward : gates = Gx[t] + h_prev W_hh^T (+ bias);  c, h = cell(gates);  activated gates saved in place.
 //   backward: dh = dY[t] + dG[t_next] W_hh ;  dG[t], dc = cell'(...)        (the GEMM feeds the cell directly)
 // =====================================================================================================
@@ -547,11 +502,12 @@ struct LstmFwdDir {
 };
 struct LstmFwdArgs { LstmFwdDir d[2]; int64_t ldh; int B, H, have_h; };
 
-// Both LSTM step kernels: 64 output columns per CTA, 2 producer/MMA warps + 16 epilogue warps (4 TMEM lane quarters x
-// 4 groups of 16 columns): the cell arithmetic is transcendental-heavy and latency-bound, so it is spread over as many
-// warps and CTAs as the tile shape allows (a 128x256 tile with 4 epilogue warps took ~27 us per step).
+// Both LSTM step kernels: 64 output columns per CTA, a producer warp, 16 epilogue warps (4 row quarters x 4 groups of 16
+// columns) and the MMA warpgroup: the cell arithmetic is transcendental-heavy and latency-bound, so it is spread over as
+// many warps and CTAs as the tile shape allows.
 constexpr int kLstmBN = 64;
-constexpr int kLstmThreads = 64 + 16 * 32;
+constexpr int kLstmMma0 = 640;                      // 64 + 16 epilogue warps, padded to a warpgroup boundary
+constexpr int kLstmThreads = kLstmMma0 + kMmaThreads;
 
 template <int STAGES>
 __global__ void __launch_bounds__(kLstmThreads, 1)
@@ -565,7 +521,6 @@ lstm_step_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
     uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
     uint64_t *empty = full + STAGES;
     uint64_t *tmem_full = empty + STAGES;
-    uint32_t *tmem_slot = (uint32_t *)(tmem_full + 1);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dir = blockIdx.z;
     const CUtensorMap *tmA = dir ? &tmA1 : &tmA0;
@@ -581,11 +536,8 @@ lstm_step_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
         mbar_init(tmem_full, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, BN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    float *acc_tile = (float *)smem;
 
     if (warp == 0) {
         if (elect_one()) {
@@ -597,31 +549,26 @@ lstm_step_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
                 tma_load_2d(tmB, full + s, smem + s * L::STAGE_BYTES + L::A_BYTES, i * BK, n0);
             }
         }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = make_idesc(BM, BN, 0, 0);
-        for (int i = 0; i < nkb; ++i) {
-            const int s = i % STAGES;
-            mbar_wait(full + s, (i / STAGES) & 1);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
-                const uint32_t b_addr = a_addr + L::A_BYTES;
+    } else if (threadIdx.x >= kLstmMma0) {
+        // ------------------------------------------------------------ MMA warpgroup
+        const int mt = threadIdx.x - kLstmMma0;
+        AccTile<BN> acc;
+        mma_ring(nkb, STAGES, full, empty, mt == 0, [&](int i, int s) {
+            const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
+            const uint32_t b_addr = a_addr + L::A_BYTES;
 #pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k)
-                    umma_bf16(tmem_base, make_desc(a_addr + k * 32, 16, 1024), make_desc(b_addr + k * 32, 16, 1024), idesc,
-                              (i | k) != 0);
-                umma_commit(empty + s);
-                if (i == nkb - 1) umma_commit(tmem_full);
-            }
-            __syncwarp();
-        }
-    } else {
-        const int qd = warp & 3, grp = (warp - 2) >> 2;       // TMEM lane quarter, 16-column group
+            for (int k = 0; k < BK / UMMA_K; ++k)
+                acc.template mma<0, 0>(make_desc(a_addr + k * 32, 16, 1024), make_desc(a_addr + 64 * 128 + k * 32, 16, 1024),
+                                       make_desc(b_addr + k * 32, 16, 1024), (i | k) != 0);
+        });
+        if (nkb > 0) mma_publish<BN>(acc, acc_tile, tmem_full, mt);
+    } else if (warp >= 2 && threadIdx.x < 64 + 16 * 32) {
+        const int qd = warp & 3, grp = (warp - 2) >> 2;       // 32-row quarter of the tile, 16-column group
         const int row = m0 + qd * 32 + lane;
-        if (nkb > 0) { mbar_wait(tmem_full, 0); tc_fence_after(); }
+        if (nkb > 0) mbar_wait(tmem_full, 0);
         const int H = a.H;
         uint32_t r[16];
-        if (nkb > 0) tmem_ld16(tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(grp * 16), r);
+        if (nkb > 0) acc_ld<16>(acc_tile, AccTile<BN>::LD, qd * 32, grp * 16, r);
         else {
 #pragma unroll
             for (int j = 0; j < 16; ++j) r[j] = 0;
@@ -680,12 +627,6 @@ lstm_step_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
             *reinterpret_cast<uint2 *>(q.h_out + (int64_t)row * a.ldh + j0) = hp;
             *reinterpret_cast<uint2 *>(q.h_next + (int64_t)row * H + j0) = hp;
         }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, BN);
     }
 }
 
@@ -711,7 +652,6 @@ lstm_step_bwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
     uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
     uint64_t *empty = full + STAGES;
     uint64_t *tmem_full = empty + STAGES;
-    uint32_t *tmem_slot = (uint32_t *)(tmem_full + 1);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dir = blockIdx.z;
     const CUtensorMap *tmA = dir ? &tmA1 : &tmA0;
@@ -727,11 +667,8 @@ lstm_step_bwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
         mbar_init(tmem_full, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, BN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    float *acc_tile = (float *)smem;
 
     if (warp == 0) {
         if (elect_one()) {
@@ -743,31 +680,26 @@ lstm_step_bwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
                 tma_load_2d(tmB, full + s, smem + s * L::STAGE_BYTES + L::A_BYTES, n0, i * BK);   // W_hh [4H, H], MN-major
             }
         }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = make_idesc(BM, BN, 0, 1);
-        for (int i = 0; i < nkb; ++i) {
-            const int s = i % STAGES;
-            mbar_wait(full + s, (i / STAGES) & 1);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
-                const uint32_t b_addr = a_addr + L::A_BYTES;
+    } else if (threadIdx.x >= kLstmMma0) {
+        // ------------------------------------------------------------ MMA warpgroup
+        const int mt = threadIdx.x - kLstmMma0;
+        AccTile<BN> acc;
+        mma_ring(nkb, STAGES, full, empty, mt == 0, [&](int i, int s) {
+            const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
+            const uint32_t b_addr = a_addr + L::A_BYTES;
 #pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k)
-                    umma_bf16(tmem_base, make_desc(a_addr + k * 32, 16, 1024), make_desc(b_addr + k * 2048, BK * 128, 1024),
-                              idesc, (i | k) != 0);
-                umma_commit(empty + s);
-                if (i == nkb - 1) umma_commit(tmem_full);
-            }
-            __syncwarp();
-        }
-    } else {
+            for (int k = 0; k < BK / UMMA_K; ++k)
+                acc.template mma<0, 1>(make_desc(a_addr + k * 32, 16, 1024), make_desc(a_addr + 64 * 128 + k * 32, 16, 1024),
+                                       make_desc(b_addr + k * 2048, BK * 128, 1024), (i | k) != 0);
+        });
+        if (nkb > 0) mma_publish<BN>(acc, acc_tile, tmem_full, mt);
+    } else if (warp >= 2 && threadIdx.x < 64 + 16 * 32) {
         const int qd = warp & 3, grp = (warp - 2) >> 2;
         const int row = m0 + qd * 32 + lane;
-        if (nkb > 0) { mbar_wait(tmem_full, 0); tc_fence_after(); }
+        if (nkb > 0) mbar_wait(tmem_full, 0);
         const int H = a.H;
         uint32_t r[16];
-        if (nkb > 0) tmem_ld16(tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(grp * 16), r);
+        if (nkb > 0) acc_ld<16>(acc_tile, AccTile<BN>::LD, qd * 32, grp * 16, r);
         else {
 #pragma unroll
             for (int j = 0; j < 16; ++j) r[j] = 0;
@@ -831,12 +763,6 @@ lstm_step_bwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
                 }
             }
         }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, BN);
     }
 }
 
@@ -846,7 +772,7 @@ int launch(const CUtensorMap &ta, const CUtensorMap &tb, const GemmArgs &g, int 
     auto kern = gemm_tcgen05_kernel<BN, STAGES, A_MN, B_MN>;
     { int rc_attr = ensure_dyn_smem((const void *)kern, L::TOTAL, "gemm_tcgen05 smem attr"); if (rc_attr) return rc_attr; }
     dim3 grid((unsigned)ceil_div(g.M, BM), (unsigned)ceil_div(g.N, BN), (unsigned)splits);
-    kern<<<grid, 192, L::TOTAL, st>>>(ta, tb, g);
+    kern<<<grid, kGemmThreads, L::TOTAL, st>>>(ta, tb, g);
     return check_launch("gemm_tcgen05_kernel");
 }
 
@@ -869,13 +795,13 @@ int make_map_nhwc(CUtensorMap *m, const void *base, int64_t C, int64_t W, int64_
     return MR_OK;
 }
 
-template <int BN, int STAGES, int MT, int TMA_A>
+template <int BN, int STAGES, int TMA_A>
 int launch_conv(const CUtensorMap &tb, const CUtensorMap *tx, const ConvArgs &a, int tiles, cudaStream_t st) {
-    using L = ConvSmem<BN, STAGES, MT>;
-    auto kern = conv_fprop_tcgen05_kernel<BN, STAGES, MT, TMA_A>;
+    using L = ConvSmem<BN, STAGES>;
+    auto kern = conv_fprop_tcgen05_kernel<BN, STAGES, TMA_A>;
     { int rc_attr = ensure_dyn_smem((const void *)kern, L::TOTAL, "conv_fprop smem attr"); if (rc_attr) return rc_attr; }
-    dim3 grid(TMA_A ? (unsigned)ceil_div(tiles, MT) : (unsigned)ceil_div(a.g.M, BM * MT), (unsigned)ceil_div(a.g.N, BN), 1);
-    kern<<<grid, 192, L::TOTAL, st>>>(tb, tx[0], tx[1], tx[2], tx[3], a);
+    dim3 grid(TMA_A ? (unsigned)tiles : (unsigned)ceil_div(a.g.M, BM), (unsigned)ceil_div(a.g.N, BN), 1);
+    kern<<<grid, kGemmThreads, L::TOTAL, st>>>(tb, tx[0], tx[1], tx[2], tx[3], a);
     return check_launch("conv_fprop_tcgen05_kernel");
 }
 
@@ -885,7 +811,7 @@ int launch_wgrad(const CUtensorMap &tdz, const CUtensorMap &tx, const WgradArgs 
     auto kern = conv_wgrad_tcgen05_kernel<BN, RB, STAGES>;
     { int rc_attr = ensure_dyn_smem((const void *)kern, L::TOTAL, "conv_wgrad smem attr"); if (rc_attr) return rc_attr; }
     dim3 grid((unsigned)ceil_div(a.g.M, BM), (unsigned)ceil_div(a.g.N, BN), (unsigned)splits);
-    kern<<<grid, 192, L::TOTAL, st>>>(tdz, tx, a);
+    kern<<<grid, kGemmThreads, L::TOTAL, st>>>(tdz, tx, a);
     return check_launch("conv_wgrad_tcgen05_kernel");
 }
 
@@ -893,7 +819,7 @@ int launch_wgrad(const CUtensorMap &tdz, const CUtensorMap &tx, const WgradArgs 
 
 extern "C" {
 
-/* bf16 GEMM on tcgen05/TMA.  transA = 0: A stored [M,K] (lda >= K); transA = 1: A stored [K,M] (lda >= M).
+/* bf16 GEMM on wgmma/TMA.  transA = 0: A stored [M,K] (lda >= K); transA = 1: A stored [K,M] (lda >= M).
  * transB = 1: B stored [N,K] (ldb >= K);  transB = 0: B stored [K,N] (ldb >= N).   [same convention as mr_gemm]
  * Supported operand forms: (transA, transB) = (0, 1) "NT", (0, 0) "NN" and (1, 0) "TN".  lda, ldb multiples of 8, bases 16-byte
  * aligned.  out_dtype 0 = fp32, 1 = bf16.  beta must be 0 or 1; beta = 1 (fp32 only) accumulates atomically and allows
@@ -912,7 +838,7 @@ int mr_gemm_tcgen05(const void *A, const void *B, void *C, int64_t M, int64_t N,
     if (splits < 1) splits = 1;
     if (splits > 1 && beta != 1.f) return MR_ERR_UNSUPPORTED;
     cudaStream_t st = (cudaStream_t)stream;
-    const int BN = N > 128 ? 256 : (N > 64 ? 128 : 64);
+    const int BN = N > 64 ? 128 : 64;
     CUtensorMap ta, tb;
     int rc;
     if (nt) {
@@ -939,7 +865,6 @@ int mr_gemm_tcgen05(const void *A, const void *B, void *C, int64_t M, int64_t N,
 #define MR_LAUNCH(BNV, STV)                                                              \
     (nt ? launch<BNV, STV, 0, 0>(ta, tb, g, splits, st)                                  \
         : (nn ? launch<BNV, STV, 0, 1>(ta, tb, g, splits, st) : launch<BNV, STV, 1, 1>(ta, tb, g, splits, st)))
-    if (BN == 256) return MR_LAUNCH(256, 4);
     if (BN == 128) return MR_LAUNCH(128, 6);
     return MR_LAUNCH(64, 8);
 #undef MR_LAUNCH
@@ -972,21 +897,17 @@ int mr_conv2d_fprop_tcgen05(const void *x, const void *Wm, void *y, int N, int H
     if (P > (1LL << 31) - 256) return MR_ERR_UNSUPPORTED;
     a.g.M = (int)P; a.g.N = Cout; a.g.K = (int)K; a.g.ldc = Cout; a.g.C = y; a.g.bias = bias; a.g.relu = relu;
     a.g.out_bf16 = out_dtype == 1; a.g.atomic = 0; a.g.kblocks_per_split = 0;
-    const int BN = Cout > 128 ? 256 : (Cout > 64 ? 128 : 64);
+    const int BN = Cout > 64 ? 128 : 64;
     CUtensorMap tb;
     int rc = make_map(&tb, Wm, K, Cout, K, BK, BN);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    /* 256-row CTAs (MT = 2) measured SLOWER than 128-row CTAs on B200 (conv5: 1186 us vs 841 us): kept selectable for
-     * experiments (MR_CONV_MT2=1), off by default. */
-    static const bool mt2 = getenv("MR_CONV_GATHER_MT2") && getenv("MR_CONV_GATHER_MT2")[0] == '1';
-    const bool big = mt2 && P >= 4 * 148 * 128;
     /* TMA-A variant: tile the output space with boxes of 128 pixels, width cut into power-of-two segments. */
     static const bool no_tma_a = getenv("MR_CONV_NO_TMA_A") != nullptr;
-    a.nseg = 0; a.ntiles = 0;
+    a.nseg = 0;
     CUtensorMap tx[4];
     int tiles = 0;
-    if (!no_tma_a && !big) {
+    if (!no_tma_a) {
         int w0 = 0;
         bool ok = true;
         while (w0 < a.Wo) {
@@ -1016,28 +937,18 @@ int mr_conv2d_fprop_tcgen05(const void *x, const void *Wm, void *y, int N, int H
              * (the kernel is not persistent); MR_CONV_SHALLOW=0/1 overrides the default for experiments. */
             static const char *sh_env = getenv("MR_CONV_SHALLOW");
             const bool shallow = sh_env ? sh_env[0] == '1' : true;
-            a.ntiles = tiles;
-            /* narrow outputs (Cout <= 128): a CTA can take TWO pixel tiles per weight tile (two TMEM accumulators,
-             * 2 x BN <= 256 columns: still two CTAs per SM), which cuts the operand bytes per FLOP by a third.  Measured
-             * NEUTRAL on the CRNN step (9.262 vs 9.266 ms): these layers are not operand-bound.  Parity-tested, selectable
-             * with MR_CONV_MT2=1, off by default. */
-            const char *mt2_env = getenv("MR_CONV_MT2");
-            const bool pair = mt2_env && mt2_env[0] == '1' && BN <= 128 && tiles >= 4 * 148;
             if (shallow) {
-                if (BN == 256) return launch_conv<256, 2, 1, 1>(tb, tx, a, tiles, st);
-                if (BN == 128) return pair ? launch_conv<128, 2, 2, 1>(tb, tx, a, tiles, st) : launch_conv<128, 3, 1, 1>(tb, tx, a, tiles, st);
-                return pair ? launch_conv<64, 2, 2, 1>(tb, tx, a, tiles, st) : launch_conv<64, 3, 1, 1>(tb, tx, a, tiles, st);
+                if (BN == 128) return launch_conv<128, 3, 1>(tb, tx, a, tiles, st);
+                return launch_conv<64, 3, 1>(tb, tx, a, tiles, st);
             }
-            if (BN == 256) return launch_conv<256, 4, 1, 1>(tb, tx, a, tiles, st);
-            if (BN == 128) return launch_conv<128, 6, 1, 1>(tb, tx, a, tiles, st);
-            return launch_conv<64, 8, 1, 1>(tb, tx, a, tiles, st);
+            if (BN == 128) return launch_conv<128, 6, 1>(tb, tx, a, tiles, st);
+            return launch_conv<64, 8, 1>(tb, tx, a, tiles, st);
         }
         a.nseg = 0;
     }
     for (int q = 0; q < 4; ++q) tx[q] = tb;
-    if (BN == 256) return big ? launch_conv<256, 3, 2, 0>(tb, tx, a, 0, st) : launch_conv<256, 4, 1, 0>(tb, tx, a, 0, st);
-    if (BN == 128) return big ? launch_conv<128, 4, 2, 0>(tb, tx, a, 0, st) : launch_conv<128, 6, 1, 0>(tb, tx, a, 0, st);
-    return big ? launch_conv<64, 5, 2, 0>(tb, tx, a, 0, st) : launch_conv<64, 8, 1, 0>(tb, tx, a, 0, st);
+    if (BN == 128) return launch_conv<128, 6, 0>(tb, tx, a, 0, st);
+    return launch_conv<64, 8, 0>(tb, tx, a, 0, st);
 }
 
 /* Implicit-GEMM weight gradient: dWm[Cout, kh*kw*C] (fp32, ACCUMULATED atomically: zero it first) from
@@ -1076,13 +987,11 @@ int mr_conv2d_wgrad_tcgen05(const void *dz, const void *x, float *dWm, int N, in
     rc = make_map_nhwc(&tx, x, C, W, H, N, RB, 1, 1, sw, 1);      /* rows are addressed one at a time: only the width strides */
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const int BN = K > 128 ? 256 : (K > 64 ? 128 : 64);
+    const int BN = K > 64 ? 128 : 64;
     if (rb80) {
-        if (BN == 256) return launch_wgrad<256, 80, 3>(tdz, tx, a, splits, st);
         if (BN == 128) return launch_wgrad<128, 80, 4>(tdz, tx, a, splits, st);
         return launch_wgrad<64, 80, 6>(tdz, tx, a, splits, st);
     }
-    if (BN == 256) return launch_wgrad<256, 64, 4>(tdz, tx, a, splits, st);
     if (BN == 128) return launch_wgrad<128, 64, 6>(tdz, tx, a, splits, st);
     return launch_wgrad<64, 64, 8>(tdz, tx, a, splits, st);
 }

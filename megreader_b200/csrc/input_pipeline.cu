@@ -39,7 +39,7 @@ __global__ void pack_labels_kernel(const unsigned char *__restrict__ text, const
 
 int blocks_for(int64_t total) {
     const int64_t b = (total + 255) / 256;
-    return (int)(b < 1 ? 1 : (b > 148 * 16 ? 148 * 16 : b));
+    return (int)(b < 1 ? 1 : (b > mr::sm_count() * 16 ? mr::sm_count() * 16 : b));
 }
 
 }  // namespace

@@ -1,14 +1,14 @@
-// Persistent bidirectional-LSTM recurrence for sm_100a (decoders/crnn.py:13,17 nn.LSTM inside BidirectionalLSTM).
+// Persistent bidirectional-LSTM recurrence for sm_90a (decoders/crnn.py:13,17 nn.LSTM inside BidirectionalLSTM).
 //
 // The recurrence h_t = cell(Gx_t + h_{t-1} W_hh^T) is T dependent steps of a small GEMM ([B,H] x [H,4H]) plus a
 // transcendental-heavy cell.  Launched step by step it is launch- and latency-bound (2 launches x T x 2 layers x
-// fwd/bwd = 520 launches of 5-10 us in the CRNN train step).  Here ONE launch runs the whole sequence of one layer,
+// fwd/bwd = 520 short launches in the CRNN train step).  Here ONE launch runs the whole sequence of one layer,
 // both directions:
 //   * the CTA grid tiles (batch rows / 128) x (gate columns / 64) x direction and stays resident for all T steps;
 //   * each CTA keeps its W_hh slice in shared memory for the whole sequence (loaded once by TMA);
-//   * per step, the h_{t-1} tile is TMA-loaded from the layer output Y itself (L2-resident), tcgen05.mma accumulates
-//     the recurrent product in TMEM, 16 epilogue warps add the x-projection, apply the cell and write h_t, c_t and
-//     the activated gates; the cell state (fwd) / its gradient (bwd) never leaves registers;
+//   * per step, the h_{t-1} tile is TMA-loaded from the layer output Y itself (L2-resident), one MMA warpgroup (wgmma)
+//     accumulates the recurrent product and publishes it as a shared-memory tile, 16 epilogue warps add the
+//     x-projection, apply the cell and write h_t, c_t and the activated gates; the cell state (fwd) / its gradient (bwd) never leaves registers;
 //   * the CTAs that share batch rows exchange h_t (fwd) / dG_t (bwd) through global memory and a monotonically
 //     increasing arrival counter per (direction, row tile): writers  st -> bar.sync -> __threadfence -> atomicAdd,
 //     readers  ld.acquire spin -> fence.proxy.async -> TMA.  All CTAs must be co-resident: the host refuses grids
@@ -16,13 +16,14 @@
 // Gate columns are UNIT-MAJOR (column 4*j + g = gate g of hidden unit j; g = i,f,g,o) as in gemm_tcgen05.cu.
 // Every wait is bounded: on timeout the CTA records an error word (flags[2*row_tiles]) and runs to completion with
 // undefined results instead of hanging the device.
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 #include <stdlib.h>
 
 namespace {
 
 constexpr int kBN = 64;                       // gate columns (fwd) / hidden units (bwd) per CTA
-constexpr int kThreads = 64 + 16 * 32;        // producer warp, MMA warp, 16 epilogue warps
+constexpr int kMma0 = 640;                    // producer warp, an idle warp, 16 epilogue warps, padded to a warpgroup boundary
+constexpr int kThreads = kMma0 + kMmaThreads; // ... and the MMA warpgroup
 constexpr int kEpiThreads = 16 * 32;
 
 __device__ __forceinline__ uint32_t ld_acquire(const unsigned *p) {
@@ -90,9 +91,6 @@ __device__ __forceinline__ void tma_store_commit_wait() {
 // 16-byte chunk `c` of row `r` in a [rows x 128 B] tile written by TMA with the 128-byte swizzle (tile base 1024-aligned)
 __device__ __forceinline__ uint32_t swz(int r, int c) { return (uint32_t)(r * 128 + ((c ^ (r & 7)) << 4)); }
 
-// byte offset `a` inside a 1024-aligned tile written / read by TMA with the 128-byte swizzle (any row pitch)
-__device__ __forceinline__ uint32_t swz_addr(uint32_t a) { return a ^ ((a >> 3) & 0x70u); }
-
 struct SeqFwdArgs {
     bf16 *G;                  // [2, T, B, 4H] unit-major: x-projection on entry, activated gates on exit
     const float *bias[2];     // [4H] unit-major, b_ih + b_hh
@@ -114,11 +112,11 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
     unsigned char *Ws = smem + nkb * 16384;               // nkb x [ 64 rows x 128 B]   W_hh slice, K-major SW128
     unsigned char *Gt = Ws + nkb * 8192;                  // 2 x [128 rows x 128 B]     gates tile: x-projection in, activations out
     unsigned char *Ct = Gt + 32768;                       // [128 rows x 64 B]          cell-state tile (16 units fp32), out
-    uint64_t *wfull = (uint64_t *)(Ct + 8192);
+    float *acc_tile = (float *)(Ct + 8192);               // [128 rows x (64 + 1)] fp32      recurrent product of this step
+    uint64_t *wfull = (uint64_t *)(Ct + 8192 + AccTile<kBN>::BYTES);
     uint64_t *afull = wfull + 1;                          // [8]
     uint64_t *tmem_full = afull + 8;
     uint64_t *gfull = tmem_full + 1;                      // [2]
-    uint32_t *tmem_slot = (uint32_t *)(gfull + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dir = blockIdx.z;
@@ -142,11 +140,7 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
         mbar_init(gfull + 1, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, kBN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == 0) {
         if (elect_one()) {
@@ -164,27 +158,31 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
                 MR_TRACE(s, 1);
             }
         }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = make_idesc(BM, kBN, 0, 0);
+    } else if (threadIdx.x >= kMma0) {
+        const int mt = threadIdx.x - kMma0;
+        if (mt != 0) trace = nullptr;
+        AccTile<kBN> acc;
         if (!mbar_wait_bounded(wfull, 0, err)) atomicExch(err, 2u);
         for (int s = 1; s < T; ++s) {
             for (int kb = 0; kb < nkb; ++kb) {
                 if (!mbar_wait_bounded(afull + kb, (s - 1) & 1, err)) atomicExch(err, 3u);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint32_t a_addr = smem_u32(As + kb * 16384), b_addr = smem_u32(Ws + kb * 8192);
+                const uint32_t a_addr = smem_u32(As + kb * 16384), b_addr = smem_u32(Ws + kb * 8192);
+                wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k)
-                        umma_bf16(tmem_base, make_desc(a_addr + k * 32, 16, 1024), make_desc(b_addr + k * 32, 16, 1024), idesc,
-                                  (kb | k) != 0);
-                    if (kb == nkb - 1) { umma_commit(tmem_full); MR_TRACE(s, 2); }
-                }
-                __syncwarp();
+                for (int k = 0; k < BK / UMMA_K; ++k)
+                    acc.mma<0, 0>(make_desc(a_addr + k * 32, 16, 1024), make_desc(a_addr + 64 * 128 + k * 32, 16, 1024),
+                                  make_desc(b_addr + k * 32, 16, 1024), (kb | k) != 0);
+                wgmma_commit();
             }
+            wgmma_wait<0>();
+            // the epilogue warps drained the previous step's tile before any peer could post the arrival this step waited for
+            acc.store(acc_tile, mt);
+            mma_group_sync();
+            if (mt == 0) { mbar_arrive(tmem_full); MR_TRACE(s, 2); }
         }
-    } else {
+    } else if (warp >= 2 && threadIdx.x < 64 + kEpiThreads) {
         if (threadIdx.x != 64) trace = nullptr;
-        const int qd = warp & 3, grp = (warp - 2) >> 2;        // TMEM lane quarter, group of 16 gate columns = 4 units
+        const int qd = warp & 3, grp = (warp - 2) >> 2;        // 32-row quarter of the tile, group of 16 gate columns = 4 units
         const int row = m0 + qd * 32 + lane;
         const int col0 = n0 + grp * 16, j0 = col0 >> 2;
         const bool live = row < B;
@@ -195,9 +193,8 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
             bb[4 * v] = b4.x; bb[4 * v + 1] = b4.y; bb[4 * v + 2] = b4.z; bb[4 * v + 3] = b4.w;
         }
         float cst[4] = {0.f, 0.f, 0.f, 0.f};
-        const uint32_t taddr = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(grp * 16);
         // The gates tile [128 rows x 64 columns] of every step comes and goes by TMA (row-per-thread global accesses
-        // cost 32 wavefronts per warp instruction, measured ~1 us per step): loaded two steps ahead into a double
+        // cost 32 wavefronts per warp instruction): loaded two steps ahead into a double
         // buffer, activated in place, stored together with the cell-state tile by the leader thread.
         const bool leader = threadIdx.x == 64;
         const int rl = qd * 32 + lane;
@@ -220,8 +217,7 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
             uint32_t r[16];
             if (s > 0) {
                 if (!mbar_wait_bounded(tmem_full, (s - 1) & 1, err)) atomicExch(err, 4u);
-                tc_fence_after();
-                tmem_ld16(taddr, r);
+                acc_ld<16>(acc_tile, AccTile<kBN>::LD, qd * 32, grp * 16, r);
             } else {
 #pragma unroll
                 for (int j = 0; j < 16; ++j) r[j] = 0;
@@ -261,7 +257,6 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
             }
             // h_t is all the peers wait for: post the arrival before the state that only the backward pass reads
             MR_TRACE(s, 4);
-            tc_fence_before();
             epi_bar_sync();                                      // every h_t of this tile stored, accumulator drained
             MR_TRACE(s, 5);
             if (threadIdx.x == 64) {
@@ -291,11 +286,6 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
             }
         }
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, kBN);
-    }
 }
 
 struct SeqBwdArgs {
@@ -308,17 +298,10 @@ struct SeqBwdArgs {
     int T, B, H;
 };
 
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t *r) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
 // Backward recurrence: dh_{t} += dG_{t_next} W_hh needs the FULL gate-gradient row block [128 x 4H] per output tile, so
 // the per-step operand traffic is (H / units-per-CTA) x the dG tile.  32 hidden units per CTA spread the step over
-// (B/128) x (H/32) x 2 CTAs (64 at the CRNN shape).  A thread owns one batch row (TMEM lane), so direct global access
-// would touch 32 different rows per warp instruction (measured: 4.4 us of an 11 us step for the operand loads alone).
+// (B/128) x (H/32) x 2 CTAs (64 at the CRNN shape).  A thread owns one batch row, so direct global access
+// would touch 32 different rows per warp instruction.
 // Instead the per-step operands -- activated gates [128 x 128] bf16 and cell state [128 x 32] fp32 -- are TMA-loaded as
 // swizzled tiles one step ahead and read conflict-free from shared memory; the gate gradients are written back into the
 // gates tile and leave through one TMA store.  c_prev of this step is the c tile of the next one: one new tile per step.
@@ -337,13 +320,13 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
     unsigned char *Gs = smem + STAGES * 16384;            // 2 x [128 x 128 B]            gates of this step -> dG of this step
     unsigned char *Cs = Gs + 32768;                       // 2 x [128 x 128 B]            cell-state tiles (fp32, 32 units)
     unsigned char *Ws = Cs + 32768;                       // nkb x [32 rows x 128 B]      W_hh^T[n0.., kb*64..), K-major SW128
-    uint64_t *wfull = (uint64_t *)(Ws + nkb * kBwdWTile);
+    float *acc_tile = (float *)(Ws + nkb * kBwdWTile);    // [128 rows x (32 + 1)] fp32    recurrent product of this step
+    uint64_t *wfull = (uint64_t *)(Ws + nkb * kBwdWTile + AccTile<kBwdBN>::BYTES);
     uint64_t *full = wfull + 1;
     uint64_t *empty = full + STAGES;
     uint64_t *tmem_full = empty + STAGES;
     uint64_t *gfull = tmem_full + 1;
     uint64_t *cfull = gfull + 1;                          // [2]
-    uint32_t *tmem_slot = (uint32_t *)(cfull + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dir = blockIdx.z;
@@ -369,11 +352,7 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
         mbar_init(cfull + 1, 1);
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, kBwdBN);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     // processing order u = 0..T-1 is the reverse of the forward order: direction 0 walks t = T-1..0, direction 1 t = 0..T-1
     if (warp == 0) {
@@ -396,32 +375,39 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
                 MR_TRACE(u, 1);
             }
         }
-    } else if (warp == 1) {
-        constexpr uint32_t idesc = make_idesc(BM, kBwdBN, 0, 0);
+    } else if (threadIdx.x >= kMma0) {
+        const int mt = threadIdx.x - kMma0;
+        if (mt != 0) trace = nullptr;
+        AccTile<kBwdBN> acc;
         if (!mbar_wait_bounded(wfull, 0, err)) atomicExch(err, 2u);
         int it = 0;
         for (int u = 1; u < T; ++u) {
+            uint64_t *pending = nullptr;
             for (int kb = 0; kb < nkb; ++kb, ++it) {
                 const int s = it % STAGES;
                 if (!mbar_wait_bounded(full + s, (it / STAGES) & 1, err)) atomicExch(err, 3u);
-                tc_fence_after();
-                if (elect_one()) {
-                    if (kb < 16) MR_TRACE(u, 8 + kb);
-                    const uint32_t a_addr = smem_u32(As + s * 16384), b_addr = smem_u32(Ws + kb * kBwdWTile);
+                if (kb < 16) MR_TRACE(u, 8 + kb);
+                const uint32_t a_addr = smem_u32(As + s * 16384), b_addr = smem_u32(Ws + kb * kBwdWTile);
+                wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; ++k)
-                        umma_bf16(tmem_base, make_desc(a_addr + k * 32, 16, 1024), make_desc(b_addr + k * 32, 16, 1024), idesc,
-                                  (kb | k) != 0);
-                    umma_commit(empty + s);
-                    if (kb == nkb - 1) { umma_commit(tmem_full); MR_TRACE(u, 2); }
-                }
-                __syncwarp();
+                for (int k = 0; k < BK / UMMA_K; ++k)
+                    acc.mma<0, 0>(make_desc(a_addr + k * 32, 16, 1024), make_desc(a_addr + 64 * 128 + k * 32, 16, 1024),
+                                  make_desc(b_addr + k * 32, 16, 1024), (kb | k) != 0);
+                wgmma_commit();
+                wgmma_wait<1>();                                 // the previous k-block has retired: its slot is free
+                if (pending && mt == 0) mbar_arrive(pending);
+                pending = empty + s;
             }
+            wgmma_wait<0>();
+            if (pending && mt == 0) mbar_arrive(pending);
+            acc.store(acc_tile, mt);
+            mma_group_sync();
+            if (mt == 0) { mbar_arrive(tmem_full); MR_TRACE(u, 2); }
         }
-    } else {
+    } else if (warp >= 2 && threadIdx.x < 64 + kEpiThreads) {
         const bool leader = threadIdx.x == 64;
         if (!leader) trace = nullptr;
-        const int qd = warp & 3, grp = (warp - 2) >> 2;        // TMEM lane quarter, group of 8 hidden units
+        const int qd = warp & 3, grp = (warp - 2) >> 2;        // 32-row quarter of the tile, group of 8 hidden units
         const int rl = qd * 32 + lane, row = m0 + rl;
         const int j0 = n0 + grp * 8;
         const bool live = row < B;
@@ -431,7 +417,6 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
         float dcs[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) dcs[j] = 0.f;
-        const uint32_t taddr = tmem_base + ((uint32_t)(qd * 32) << 16) + (uint32_t)(grp * 8);
         auto time_of = [&](int u) { return dir ? u : T - 1 - u; };
         auto load_gates = [&](int u) {
             const int z = dir * T + time_of(u);
@@ -470,8 +455,7 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
             uint32_t r[8];
             if (u > 0) {
                 if (!mbar_wait_bounded(tmem_full, (u - 1) & 1, err)) atomicExch(err, 4u);
-                tc_fence_after();
-                tmem_ld8(taddr, r);
+                acc_ld<8>(acc_tile, AccTile<kBwdBN>::LD, qd * 32, grp * 8, r);
             } else {
 #pragma unroll
                 for (int j = 0; j < 8; ++j) r[j] = 0;
@@ -512,7 +496,6 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
             }
             fence_proxy_async();                                 // generic-proxy tile writes -> visible to the TMA store
             MR_TRACE(u, 4);
-            tc_fence_before();
             epi_bar_sync();
             MR_TRACE(u, 5);
             if (leader) {
@@ -529,11 +512,6 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
                 if (u + 2 < T) load_cell(u + 2);                 // into the buffer that held c_t of this step
             }
         }
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, kBwdBN);
     }
 }
 
@@ -599,11 +577,12 @@ int mr_lstm_seq_set_trace(void *buf) { g_trace = (long long *)buf; return MR_OK;
 /* Whole-sequence recurrence of one bidirectional LSTM layer, forward.  See include/megreader_b200.h. */
 int mr_lstm_seq_fwd_tcgen05(const void *const *Whh, void *G, const float *const *bias, float *C, void *Y,
                             unsigned *flags, int T, int B, int H, void *stream) {
-    if (T <= 0 || B <= 0 || H <= 0 || H % 64 || H > 512) return MR_ERR_UNSUPPORTED;
+    if (T <= 0 || B <= 0 || H <= 0 || H % 64) return MR_ERR_UNSUPPORTED;
     if (!Whh || !Whh[0] || !Whh[1] || !G || !bias || !bias[0] || !bias[1] || !C || !Y || !flags) return MR_ERR_NULL_POINTER;
     if ((int64_t)2 * T * B >= (int64_t)1 << 31) return MR_ERR_UNSUPPORTED;
     const int nkb = H / BK, row_tiles = ceil_div(B, BM);
-    const size_t smem = (size_t)nkb * (16384 + 8192) + 32768 + 8192 + 16 * 8 + 1024;
+    const size_t smem = (size_t)nkb * (16384 + 8192) + 32768 + 8192 + AccTile<kBN>::BYTES + 16 * 8 + 1024;
+    if (nkb > 8 || smem > 227 * 1024) return MR_ERR_UNSUPPORTED;      /* afull[8]; in practice shared memory allows H <= 384 */
     auto kern = lstm_seq_fwd_kernel;
     { int rc_attr = ensure_dyn_smem((const void *)kern, smem, "lstm seq fwd smem attr"); if (rc_attr) return rc_attr; }
     dim3 grid((unsigned)row_tiles, (unsigned)(4 * H / kBN), 2);
@@ -637,7 +616,7 @@ int mr_lstm_seq_bwd_tcgen05(const void *const *WhhT, const void *G, const float 
     if (!WhhT || !WhhT[0] || !WhhT[1] || !G || !C || !dY || !dG || !flags) return MR_ERR_NULL_POINTER;
     if ((int64_t)2 * T * B >= (int64_t)1 << 31) return MR_ERR_UNSUPPORTED;
     const int nkb = 4 * H / BK, row_tiles = ceil_div(B, BM);
-    const size_t smem = (size_t)kBwdStages * 16384 + 65536 + (size_t)nkb * kBwdWTile + (2 * kBwdStages + 8) * 8 + 1024;
+    const size_t smem = (size_t)kBwdStages * 16384 + 65536 + (size_t)nkb * kBwdWTile + AccTile<kBwdBN>::BYTES + (2 * kBwdStages + 8) * 8 + 1024;
     if (smem > 227 * 1024) return MR_ERR_UNSUPPORTED;
     auto kern = lstm_seq_bwd_kernel<kBwdStages>;
     { int rc_attr = ensure_dyn_smem((const void *)kern, smem, "lstm seq bwd smem attr"); if (rc_attr) return rc_attr; }

@@ -1,13 +1,12 @@
-// NHWC building blocks of the CRNN training engine (sm_100a): layout conversion, im2col / col2im, fused
+// NHWC building blocks of the CRNN training engine (sm_90a): layout conversion, im2col / col2im, fused
 // bias+ReLU+max-pool (forward and backward), training-mode BatchNorm (stats / apply / backward), column sums,
 // LSTM cell (forward / backward), fused Adam, weight layout packs, greedy CTC decoders.  All HBM-bound streaming
 // kernels: 16-byte vector accesses along the channel dimension, fp32 accumulation; per-channel sums leave each block
 // as one row of an fp32 partial buffer and are added in double by a small second kernel (no atomics on the hot path).
 //
 // Why these exist: with the ATen/cuDNN composition of the reference's modules (backbones/crnn.py:46-55,
-// decoders/crnn.py:8-24) the tensor-core convolutions are ~12 % of a B200 training step; NCHW max-pool forward /
-// backward, NCHW<->NHWC transposes, BatchNorm and the per-timestep LSTM glue are the other 88 %
-// (profiles/r1_library_step_launches.md).  Keeping activations NHWC end to end and fusing the elementwise chains
+// decoders/crnn.py:8-24) the tensor-core convolutions are a small part of a training step; NCHW max-pool forward /
+// backward, NCHW<->NHWC transposes, BatchNorm and the per-timestep LSTM glue are most of it.  Keeping activations NHWC end to end and fusing the elementwise chains
 // removes that traffic.
 //
 // dtype codes: 0 = float32, 1 = bfloat16.  "rows" = N*H*W pixels, C = channels (innermost).
@@ -80,7 +79,7 @@ __device__ __forceinline__ void block_channel_sum(const float *acc, int cv, doub
 
 // Same reduction without atomics: every block stores its per-channel sums as one row of a [gridDim.x, C] fp32 scratch;
 // partials_finalize_kernel adds the rows in double.  (fp64 atomics from thousands of blocks onto C addresses serialise
-// at ~40 ns each: measured 150-200 us per launch for C = 512 and a 4736-block grid, more than the streaming itself.)
+// and cost more than the streaming itself.)
 template <int VN>
 __device__ __forceinline__ void block_channel_partial(const float *acc, int cv, float *part_row, float (*red)[VN + 1]) {
 #pragma unroll
@@ -99,7 +98,7 @@ __device__ __forceinline__ void block_channel_partial(const float *acc, int cv, 
 }
 
 // out[c] = sum_b part[b, c] (double).  Block = 32 columns x 32 row lanes: each lane walks rows lane, lane+32, ... with
-// four loads in flight (a one-thread-per-column loop over ~1000 rows is a 50 us latency chain), then a shared-memory
+// four loads in flight (a one-thread-per-column loop over ~1000 rows is one long latency chain), then a shared-memory
 // reduction over the lanes.
 __global__ void __launch_bounds__(1024)
 partials_finalize_kernel(const float *__restrict__ part, int nb, int ncols, double *__restrict__ out) {
@@ -126,7 +125,7 @@ partials_finalize_kernel(const float *__restrict__ part, int nb, int ncols, doub
     }
 }
 
-constexpr int kMaxPartialBlocks = 148 * 8;
+constexpr int kMaxPartialBlocks = 132 * 8;        // sizes a scratch buffer: 8 blocks per SM of an H100 SXM
 constexpr int kMaxPartialCols = 4096;     // 2 * C columns of statistics for C up to 2048 (ResNet-50 layer4)
 // Library-owned scratch for the block partial sums (stream-ordered use on one stream at a time).  Allocated on first
 // use, which must not happen inside a CUDA-graph capture: callers run one eager step before capturing (as they must
@@ -1020,7 +1019,7 @@ bn_apply_rows_kernel(const T *__restrict__ x, const float *__restrict__ bias, co
 
 // rows per block for a one-wave grid of `per_sm` blocks per SM, rounded to the row step of the row-tiled kernels
 inline int64_t rows_per_block(int64_t rows, int row_step, int per_sm, int *grid) {
-    int64_t rpc = ceil_div(rows, (int64_t)148 * per_sm);
+    int64_t rpc = ceil_div(rows, (int64_t)mr::sm_count() * per_sm);
     rpc = ceil_div(rpc, (int64_t)row_step) * row_step;
     *grid = (int)ceil_div(rows, rpc);
     return rpc;
@@ -1058,7 +1057,7 @@ __global__ void conv_weight_pack_kernel(const float *__restrict__ w, int Cout, i
     }
 }
 
-// LSTM gate rows between the reference's gate-major order (row g*H + j) and the unit-major order of the tcgen05 kernels
+// LSTM gate rows between the reference's gate-major order (row g*H + j) and the unit-major order of the wgmma kernels
 // (row 4*j + g): out[r, :] = a[src(r), :] (+ b[src(r), :]);  inverse = 0: unit-major <- gate-major, 1: the way back.
 template <typename T>
 __global__ void gate_rows_permute_kernel(const float *__restrict__ a, const float *__restrict__ b, int H, int cols, int inverse,
@@ -1338,7 +1337,7 @@ int mr_bias_relu_pool_fwd(const void *x, const float *bias, int N, int H, int W,
     const int vn = dtype == 0 ? 4 : 8;
     const int sft = pow2_shift(C / vn);
     if (kh == 2 && kw == 2 && sft >= 0 && sft <= 8 && (int64_t)N * H * W < ((int64_t)1 << 31)) {
-        const int nblocks = (int)std::min<int64_t>((int64_t)N * g.Ho, 148 * 16);
+        const int nblocks = (int)std::min<int64_t>((int64_t)N * g.Ho, mr::sm_count() * 16);
         DISPATCH(dtype, (pool_fwd_rows_kernel<T, 2, 2><<<nblocks, 256, 0, st>>>(g, (const T *)x, bias, (T *)y, idx, sft)));
         return check_launch("pool_fwd_rows_kernel");
     }
@@ -1414,7 +1413,7 @@ static int launch_reduce(int mode, int dtype, const void *a, const void *b, cons
     const int vn = dtype == 0 ? 4 : 8;
     const int cv = C / vn;
     const int gx = (int)ceil_div(cv, 32);
-    int64_t gy = (148 * 8) / gx;
+    int64_t gy = (mr::sm_count() * 8) / gx;
     if (gy < 1) gy = 1;
     int64_t rpc = ceil_div(rows, gy);
     if (rpc < 64) rpc = 64;

@@ -30,8 +30,8 @@ class FlatGrads:
     """The gradients of `params` as views into ONE flat fp32 buffer, in the given order (pass the parameters in backward order --
     decoder first -- and `buckets` > 1 to let the early buckets' all-reduce run while the rest of the backward is still computing).
 
-    Round 1 flattened, reduced, divided and copied back every step (~40 un-captured launches between two CUDA graphs: the
-    measured 8-GPU step grew from 8.8 to 11.4 ms although the 33 MB transfer itself is ~0.1 ms on NVSwitch).  Here autograd
+    Flattening, reducing, dividing and copying back every step costs ~40 un-captured launches between two CUDA graphs, far
+    more than the 33 MB transfer itself.  Here autograd
     accumulates straight into the views (`zero()` is one memset and keeps them attached), the collective is ONE in-place NCCL
     all-reduce with the AVG op (no separate divide) per bucket, and the optimizer reads the same views: no copies at all."""
 

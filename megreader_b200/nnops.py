@@ -141,9 +141,8 @@ def cast(x, dtype):
     return y
 
 
-# bf16 GEMMs of the engine: "tc" = the repo's tcgen05 kernel (csrc/gemm_tcgen05.cu) wherever it covers the form, "cublas" = library
-# Default "cublas": measured on the cfg-2 step (profiles/r2_gemm_routing.md) 8.95 ms with library GEMMs for the LSTM projections /
-# Linear / conv0 / weight gradients, 9.34 ms with the tcgen05 kernel on the large NT / NN forms, 10.46 ms on all forms.
+# bf16 GEMMs of the engine: "tc" = the repo's wgmma kernel (csrc/gemm_tcgen05.cu) wherever it covers the form, "cublas" = library
+# Default "cublas" for the LSTM projections / Linear / conv0 / weight gradients; the routing has not been re-measured on H100.
 GEMM_BACKEND = __import__("os").environ.get("MEGREADER_B200_GEMM", "cublas")
 GEMM_POLICY = __import__("os").environ.get("MEGREADER_B200_GEMM_POLICY", "big")      # "big" | "all"
 
@@ -153,8 +152,7 @@ def _gemm_tc_try(A, B, out, M, N, K, transA, transB, alpha, beta):
     if alpha != 1.0 or (transA and transB):
         return False
     if GEMM_POLICY == "big" and (transA or K < 256 or N < 128):
-        return False      # measured (profiles/r2_gemm_routing.md): the K = 32 conv0 GEMM and the split-K weight-gradient forms are
-                          # slower on the hand-written kernel than on the library one; they stay library GEMMs
+        return False      # the K = 32 conv0 GEMM and the split-K weight-gradient forms stay library GEMMs
     lib = _lib.lib()
     if transA:
         # weight-gradient form dW[M,N] = A^T B over a long K: split-K with fp32 atomic accumulation into a zeroed output
@@ -181,7 +179,7 @@ def _gemm_tc_try(A, B, out, M, N, K, transA, transB, alpha, beta):
 
 def gemm(A, B, transA=False, transB=False, out=None, out_dtype=None, alpha=1.0, beta=0.0):
     """Row-major out[M,N] = alpha * op(A) op(B) + beta * out.  A, B: 2-D, unit inner stride (row stride = ld).  bf16 operands go
-    to the tcgen05 kernel when it covers the form (NT / NN, TN with fp32 output); everything else is a plain library GEMM."""
+    to the wgmma kernel when it covers the form (NT / NN, TN with fp32 output); everything else is a plain library GEMM."""
     assert A.dim() == 2 and B.dim() == 2 and A.stride(1) == 1 and B.stride(1) == 1 and A.dtype == B.dtype
     M, K = (A.size(1), A.size(0)) if transA else (A.size(0), A.size(1))
     Kb, N = (B.size(1), B.size(0)) if transB else (B.size(0), B.size(1))
@@ -228,7 +226,7 @@ def adam_step(p, g, m, v, lr, beta1, beta2, eps, step, grad_scale=1.0, shadow=No
 
 
 def gemm_tc(A, B, transA=False, transB=True, out=None, out_dtype=None, bias=None, relu=False, beta=0.0, splits=1):
-    """Hand-written tcgen05/TMA bf16 GEMM (csrc/gemm_tcgen05.cu).  Same storage convention as gemm(); forms NT / TN.
+    """Hand-written wgmma/TMA bf16 GEMM (csrc/gemm_tcgen05.cu).  Same storage convention as gemm(); forms NT / TN.
     Raises MegReaderB200Error(MR_ERR_UNSUPPORTED) for shapes it does not cover."""
     assert A.dim() == 2 and B.dim() == 2 and A.stride(1) == 1 and B.stride(1) == 1
     assert A.dtype == torch.bfloat16 and B.dtype == torch.bfloat16
@@ -283,8 +281,7 @@ def conv2d_fprop_tc(x, Wm, kh, kw, sh, sw, ph, pw, dh, dw, out_dtype=torch.bfloa
     return y, Ho, Wo
 
 
-# minimum 64-pixel k-blocks per split of conv2d_wgrad_tc.  Measured on the ResNet50-PPM step (bench.py --config 3, ms per step):
-# 1: 14.06, 8: 13.41, 16: 12.46, 32: 12.78, 64: 13.03
+# minimum 64-pixel k-blocks per split of conv2d_wgrad_tc (MR_WGRAD_MIN_KB; not re-tuned on H100)
 _WGRAD_MIN_KB = max(1, int(os.environ.get("MR_WGRAD_MIN_KB", "16")))
 
 
@@ -297,7 +294,7 @@ def conv2d_wgrad_tc(dz, x, kh, kw, sh, sw, ph, pw, dh, dw, splits=0, out=None):
     if splits <= 0:
         tiles = ((Cout + 127) // 128) * ((K + 255) // 256)
         splits = max(1, -(-288 // tiles))
-        # a split should own enough 64-pixel k-blocks to amortise its fixed cost (TMEM / pipeline set-up and the fp32 atomic
+        # a split should own enough 64-pixel k-blocks to amortise its fixed cost (pipeline set-up and the fp32 atomic
         # epilogue of a whole output tile): small weights over many pixels (layer1 of a ResNet) otherwise spend their time in atomics
         kb_total = dz.size(0) * dz.size(1) * -(-dz.size(2) // 64)
         splits = max(1, min(splits, kb_total // _WGRAD_MIN_KB))

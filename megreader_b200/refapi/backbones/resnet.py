@@ -13,7 +13,7 @@ What the reference's trunk is (and what this file therefore reproduces, quirks i
   * `dilations=` only reaches the 1x1 downsample conv (resnet.py:233), where it is a no-op.
   * weight init: conv ~ N(0, sqrt(2/(k*k*cout))), BN weight 1 / bias 0 (resnet.py:215-221).
 
-The deformable units run on the sm_100a DCN kernels through `assets.ops.dcn` (megreader_b200.dcn); the
+The deformable units run on the sm_90a DCN kernels through `assets.ops.dcn` (megreader_b200.dcn); the
 dense convolutions are library calls here — this trunk is a "next" row (SURVEY.md §8 A10), not the
 measured hot path.
 """

@@ -4,7 +4,7 @@ encode = the same 7-conv / 3-pool stack as the attention head; pred_conv = 1x1 c
 train: log_softmax over classes, first feature row, (W,N,C) -> CTC with `input_lengths = 32` for every sample,
 mean reduction ( mean_b nll_b / max(len_b,1) ), no zero_infinity; returns (loss, log_probs as (N,C,W)).
 eval: softmax over classes, (N,C,H,W).
-The loss runs on the sm_100a 1-D CTC kernels (megreader_b200.ctc1d) fused with the log-softmax."""
+The loss runs on the sm_90a 1-D CTC kernels (megreader_b200.ctc1d) fused with the log-softmax."""
 import torch
 import torch.nn as nn
 import torch.nn.functional as F

@@ -2,7 +2,7 @@
 convolutions (x4 up-sampling), a 1-channel heat-map and an 8-channel dense-box 1x1 prediction, BCE-with-logits / MSE losses
 weighted per pixel and averaged per sample.  State-dict keys: head_layer.{0,1,3,4,6}.*, heatmap_pred_layer.0.*,
 densebox_pred_layer.0.*.  The stride-1 convolutions are ordinary nn.Conv2d modules, i.e. megreader_b200.conv_engine can put them on
-the tcgen05 kernels; the transposed convolutions and the element-wise losses are library (ATen) calls."""
+the wgmma kernels; the transposed convolutions and the element-wise losses are library (ATen) calls."""
 import torch
 import torch.nn as nn
 import torch.nn.functional as F

@@ -6,8 +6,7 @@ oracle/_ref/ so that the GPU parity tests can compare kernel against kernel (SUR
 TEST INFRASTRUCTURE, never on the product path.  Nothing is copied from the reference: nvcc / g++ read the sources in
 place; the only additions are the force-included oracle/ref_shim/compat.h (AT_CHECK -> TORCH_CHECK, the
 DeprecatedTypeProperties overload AT_DISPATCH needs) and an empty <THC/THC.h>.  The build needs /root/reference and the
-torch headers, i.e. it runs in the build container; the GPU box only loads the prebuilt .so files (git-ignored, shipped
-with the gpurun snapshot).  load(name) returns the pybind module or None when the .so is absent.
+torch headers; a machine without the reference only loads the prebuilt .so files (git-ignored).  load(name) returns the pybind module or None when the .so is absent.
 """
 import importlib.util
 import os
@@ -19,7 +18,7 @@ SHIM = os.path.join(HERE, "ref_shim")
 REF = os.environ.get("MEGREADER_REFERENCE", "/root/reference")
 
 # The reference launches its 2D-CTC kernels with 1024 threads per block (ctc2d_cuda_kernel.cu:16 CUDA_NUM_THREADS); the
-# fp64 instantiations need more than 64 registers per thread when compiled for sm_100 and then fail to launch ("too many
+# fp64 instantiations need more than 64 registers per thread when compiled for recent architectures and then fail to launch ("too many
 # resources requested").  Capping the register count is a compiler flag, not a source change.
 EXTRA_NVCC = {"ref_ctc2d": ["--maxrregcount=64"]}
 
@@ -39,8 +38,8 @@ def so_path(name):
 def build(verbose=False):
     """Compile every op whose .so is missing.  Returns {name: path}; raises if the reference tree is absent."""
     if not os.path.isdir(REF):
-        raise RuntimeError("reference tree %s not present: oracle/_ref can only be built in the build container" % REF)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+        raise RuntimeError("reference tree %s not present: oracle/_ref can only be built next to it" % REF)
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     from torch.utils import cpp_extension
     compat = os.path.join(SHIM, "compat.h")
     built = {}

@@ -1,7 +1,7 @@
 """ORACLE — TEST INFRASTRUCTURE ONLY.  CPU restatement ("port") of the reference's CRNN recognition path in plain
-PyTorch, used (a) as the parity checker where /root/reference is absent (GPU box) and (b) as the CPU arm of
+PyTorch, used (a) as the parity checker where the reference tree is absent and (b) as the CPU arm of
 bench.py (`--impl reference`, `cpu_baseline`).  It is validated bit-for-bit against the UNMODIFIED reference
-modules in the build container by tests/test_oracle_crnn.py.
+modules by tests/test_oracle_crnn.py.
 
   CRNNBackbonePort  <- backbones/crnn.py:4-63   (7 conv blocks; BN blocks have no ReLU, :51-54)
   BiLSTMPort        <- decoders/crnn.py:8-24

@@ -5,7 +5,7 @@ decoders/ctc_decoder2d.py:37-45, on the conv branches' raw outputs.
     cls_logits  [N,C,H,W]  -> classify = softmax(dim=1)                      (:41)
     pred = log(max(mask * classify, tiny)).permute(3,2,0,1).contiguous()     (:43-45)  -> (W,H,N,C)
 
-Pinned by tests/golden/ctc2d_head_ref.npz, which oracle/make_golden.py produced by running the UNMODIFIED reference
+Pinned by tests/golden/ctc2d_head_ref_*.npz, which oracle/make_golden.py produced by running the UNMODIFIED reference
 module's forward (its `ctc_loss` attribute replaced by a fixed linear functional so that an arbitrary upstream
 gradient reaches `pred`)."""
 import torch

@@ -10,7 +10,7 @@ cv2.resize is third-party (OpenCV 4.13 in this image, INTER_LINEAR on CV_32F): i
 `resize_bilinear_f32` — half-pixel centres, coefficients computed from scale = 1/(dst/src) in double and stored as float,
 left/right neighbours clamped by forcing the fraction to 0, rows clamped by index.  Pinned by tests/test_oracle_input.py
 against cv2 itself (<= 1e-4 on the 0..255 scale: OpenCV's SIMD path fuses some multiply-adds) and against the UNMODIFIED
-reference processes run in the build container (goldens tests/golden/input_ref.npz)."""
+reference processes (goldens tests/golden/input_ref.npz)."""
 import numpy as np
 
 RGB_MEAN = np.array([122.67891434, 116.66876762, 104.00698793])          # normalize_image.py:8

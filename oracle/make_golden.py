@@ -1,4 +1,4 @@
-"""Generate tests/golden/*.npz from the UNMODIFIED reference (build container only).
+"""Generate tests/golden/*.npz from the UNMODIFIED reference (needs the reference tree).
 
 Run:  python -m oracle.make_golden            (from the repo root; needs /root/reference)
 
@@ -213,7 +213,8 @@ def make_head():
                     tag + ".grad_cls_logits": captured["cls_logits"].grad.numpy()})
         print("head", tag, tuple(pred.shape), "tiny", dec.saved_tiny.item(), "clamped fraction",
               float((pred <= float(np.log(dec.saved_tiny.item())) + 1e-6).float().mean()))
-    np.savez_compressed(os.path.join(GOLD, "ctc2d_head_ref.npz"), **out)
+    for tag in sorted({k.split(".")[0] for k in out}):      # one file per case: each stays well under 1 MB
+        np.savez_compressed(os.path.join(GOLD, "ctc2d_head_ref_%s.npz" % tag), **{k: v for k, v in out.items() if k.startswith(tag + ".")})
 
 
 def make_input():

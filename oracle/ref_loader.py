@@ -1,4 +1,4 @@
-"""Import the UNMODIFIED reference modules from /root/reference (build container only).
+"""Import the UNMODIFIED reference modules from the reference tree (MEGREADER_REFERENCE, default /root/reference).
 
 The reference's third-party deps (tensorboardX, apex, anyconfig, ...) are not installed, so
 stub modules are injected into sys.modules first.  /root/reference does not exist on the GPU

@@ -1,9 +1,10 @@
-"""CPU (build container): the reference's three recognition yamls build UNCHANGED on megreader_b200's surfaces.
+"""CPU, where the reference tree is present: the reference's three recognition yamls build UNCHANGED on megreader_b200's surfaces.
 
 The reference's own structure/model.py (BasicModel :16-24, SequenceRecognitionModel :160-181) and concern/charsets.py are imported
-from /root/reference; `getattr(backbones, name)` / `getattr(decoders, name)` (structure/model.py:20-21) then resolve to
+from the reference tree; `getattr(backbones, name)` / `getattr(decoders, name)` (structure/model.py:20-21) then resolve to
 megreader_b200/refapi.  The state dict (names and shapes: what checkpoints hold) must equal the one the reference's own modules
-produce for the same yaml.  Skipped where /root/reference is absent (GPU box)."""
+produce for the same yaml.  What it exercises is the reference's own builder and yaml files, so it is skipped where the
+reference tree is absent; the per-module state dicts are compared anywhere by tests/test_surfaces_cpu.py."""
 import json
 import os
 import subprocess

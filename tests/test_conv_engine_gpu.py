@@ -1,4 +1,4 @@
-"""GPU: the general tcgen05 convolution (stride, dilation, 1x1 / 3x3 / stem) behind megreader_b200.conv_engine against
+"""GPU: the general wgmma convolution (stride, dilation, 1x1 / 3x3 / stem) behind megreader_b200.conv_engine against
 torch's conv2d in fp32 on the same bf16-rounded operands -- forward, input gradient, weight gradient, bias gradient -- at the
 geometries of the ResNet-50 / dilated / PPM / FPN trunks and the 2D-CTC head (SURVEY.md section 8 rows A4, A10)."""
 import pytest

@@ -1,4 +1,4 @@
-"""GPU: implicit-GEMM convolution kernels (tcgen05 + TMA + cp.async gather, csrc/gemm_tcgen05.cu) against PyTorch's
+"""GPU: implicit-GEMM convolution kernels (wgmma + TMA + cp.async gather, csrc/gemm_tcgen05.cu) against PyTorch's
 fp32 conv2d / autograd on bf16-rounded inputs."""
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a 2D-CTC kernels (through the C-ABI) against the CPU oracle on the same seeded
+"""GPU parity: the sm_90a 2D-CTC kernels (through the C-ABI) against the CPU oracle on the same seeded
 inputs, against the committed golden vectors, and through size-independent properties at full size."""
 import glob
 import os

@@ -5,12 +5,12 @@ import os
 import numpy as np
 import pytest
 import torch
+from tests.cases import load_head_golden
 
 from megreader_b200 import ctc2d, ctc2d_head
 from oracle import head_port
 
 pytestmark = pytest.mark.gpu
-GOLD = os.path.join(os.path.dirname(__file__), "golden", "ctc2d_head_ref.npz")
 
 
 def _close(a, ref, what, tol=2e-5):
@@ -26,7 +26,7 @@ def _mismatch_fraction(a, ref, tol=1e-4):
 
 @pytest.mark.parametrize("tag", ["a", "b", "c"])
 def test_against_reference_golden(cuda, tag):
-    g = np.load(GOLD)
+    g = load_head_golden()
     m = torch.from_numpy(g[tag + ".mask_logits"]).to(cuda).requires_grad_(True)
     z = torch.from_numpy(g[tag + ".cls_logits"]).to(cuda).requires_grad_(True)
     tiny = float(g[tag + ".tiny"])

@@ -1,4 +1,4 @@
-"""GPU parity: deformable conv v1/v2 (sm_100a kernels + cuBLAS fp32 GEMM through the C-ABI) against the CPU oracle
+"""GPU parity: deformable conv v1/v2 (sm_90a kernels + cuBLAS fp32 GEMM through the C-ABI) against the CPU oracle
 (oracle/dcn_oracle.c, float64) on the same seeded inputs, including the reference's stride-2 offset quirk."""
 import numpy as np
 import pytest
@@ -18,7 +18,7 @@ CASES = [
     (8, 128, 16, 16, 128, 3, 1, 1, 1, 1, 1, True, False),   # Bottleneck-like (layer2 channels, small map)
     (2, 4, 7, 9, 6, 3, 1, 1, 1, 1, 1, False, False),         # DCNv1
     (4, 8, 6, 6, 4, 3, 1, 1, 1, 2, 1, False, False),         # DCNv1 grouped
-    (2, 64, 13, 19, 128, 3, 2, 1, 1, 1, 1, True, True),      # fused tcgen05 forward + weight gradient: stride 2, ragged tiles
+    (2, 64, 13, 19, 128, 3, 2, 1, 1, 1, 1, True, True),      # fused wgmma forward + weight gradient: stride 2, ragged tiles
     (2, 128, 13, 19, 128, 3, 2, 1, 1, 1, 1, True, True),     # + fused data gradient (C % 128 == 0)
     (1, 256, 11, 18, 128, 3, 1, 1, 1, 1, 1, True, False),    # two 128-channel chunks per tap, ragged tiles
     (3, 128, 9, 21, 128, 3, 1, 2, 2, 1, 1, False, False),    # fused path, DCNv1 (no mask), dilation 2

@@ -1,4 +1,4 @@
-"""GPU: the hand-written tcgen05 + TMA GEMM (csrc/gemm_tcgen05.cu) against a plain PyTorch fp32 reference of the same
+"""GPU: the hand-written wgmma + TMA GEMM (csrc/gemm_tcgen05.cu) against a plain PyTorch fp32 reference of the same
 product on bf16-rounded inputs (fp32 accumulation both sides: tolerance covers summation order only)."""
 import pytest
 import torch

@@ -198,7 +198,7 @@ def _bilstm_run(m, x, dout, mode):
 @pytest.mark.parametrize("mode", ["step", "seq"])
 @pytest.mark.parametrize("shape", [(6, 150, 64, 64, 40), (9, 512, 128, 256, 38), (1, 7, 64, 64, 8)])
 def test_bilstm_fused_tcgen05_paths(cuda, mode, shape):
-    """H % 64 == 0 in bf16 mode: per-step fused tcgen05 kernels ("step") and the persistent whole-sequence kernels
+    """H % 64 == 0 in bf16 mode: per-step fused wgmma kernels ("step") and the persistent whole-sequence kernels
     ("seq", csrc/lstm_seq_tcgen05.cu) against nn.LSTM + nn.Linear in fp32."""
     from megreader_b200 import crnn_engine
     m, x, dout, ref, ref_dx, ref_grads = _bilstm_case(cuda, *shape, seed=6)

@@ -6,15 +6,15 @@ import os
 import numpy as np
 import pytest
 import torch
+from tests.cases import load_head_golden
 
 from oracle import head_port
 
-GOLD = os.path.join(os.path.dirname(__file__), "golden", "ctc2d_head_ref.npz")
 
 
 @pytest.mark.parametrize("tag", ["a", "b", "c"])
 def test_head_port_reproduces_reference(tag):
-    g = np.load(GOLD)
+    g = load_head_golden()
     m, z = torch.from_numpy(g[tag + ".mask_logits"]), torch.from_numpy(g[tag + ".cls_logits"])
     tiny = float(g[tag + ".tiny"])
     pred = head_port.head_log_probs(m, z, tiny)

@@ -1,5 +1,11 @@
-"""CPU: the ATen-composed surfaces of megreader_b200.refapi (SURVEY.md §8 A9/A10) reproduce the reference goldens, and —
-where /root/reference is present — carry the reference's exact state-dict keys/shapes, deformable trunk included."""
+"""CPU: the ATen-composed surfaces of megreader_b200.refapi (SURVEY.md §8 A9/A10) reproduce the reference goldens and carry the
+reference's exact state-dict keys/shapes, deformable trunk included (names, shapes and the EAST head's outputs recorded from the
+unmodified reference by oracle/make_ref_golden_cpu.py; compared with it live as well where the reference tree is present)."""
+import gzip
+import json
+import os
+
+import numpy as np
 import pytest
 import torch
 
@@ -29,7 +35,69 @@ def _keys(m):
     return [(k, tuple(v.shape)) for k, v in m.state_dict().items()]
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="/root/reference not present")
+GOLD = os.path.join(os.path.dirname(__file__), "golden")
+
+
+def test_state_dict_keys_equal_stored_reference_keys():
+    import sys
+    import types
+    import megreader_b200.refapi.backbones as mb
+    import megreader_b200.refapi.decoders as md
+    import megreader_b200.refapi.backbones.resnet as mres
+    from megreader_b200 import dcn as mdcn
+    from megreader_b200 import deform_pool as mpool
+    with gzip.open(os.path.join(GOLD, "ref_state_keys.json.gz"), "rt") as f:
+        ref = json.load(f)["modules"]
+    stored = lambda name: [(k, tuple(shape)) for k, shape in ref[name]]  # noqa: E731
+    shim = types.ModuleType("assets.ops.dcn")
+    shim.ModulatedDeformConv, shim.DeformConv = mdcn.ModulatedDeformConv, mdcn.DeformConv
+    saved = sys.modules.get("assets.ops.dcn")
+    sys.modules["assets.ops.dcn"] = shim
+    try:
+        mine = mres.deformable_resnet50(pretrained=False)
+        mine_v1 = mres.ResNet(mres.BasicBlock, [1, 1, 1, 1], dcn=dict(modulated=False, deformable_groups=2))
+    finally:
+        if saved is not None:
+            sys.modules["assets.ops.dcn"] = saved
+        else:
+            del sys.modules["assets.ops.dcn"]
+    ours = {"resnet34": mb.resnet34(pretrained=False), "resnet101": mb.resnet101(pretrained=False),
+            "Resnet34FPN": mb.Resnet34FPN(resnet_pretrained=False), "resnet50dilated_ppm_128": mb.resnet50dilated_ppm(inner_channels=128),
+            "AttentionDecoder": md.AttentionDecoder(64, inner_channels=128, max_size=16, height=2),
+            "CTCDecoder": md.CTCDecoder(64, inner_channels=96), "EASTDecoder": md.EASTDecoder(channels=64),
+            "deformable_resnet50": mine, "resnet_v1_dcn": mine_v1}
+    for cls in ("DeformRoIPoolingPack", "ModulatedDeformRoIPoolingPack"):
+        ours[cls] = getattr(mpool, cls)(0.5, 3, 8, False, trans_std=0.1, deform_fc_channels=32)
+    for name, m in ours.items():
+        assert _keys(m) == stored(name), name
+    geo = [[n, list(c.stride), list(c.dilation), list(c.padding)] for n, c in mb.resnet50dilated_ppm().named_modules()
+           if isinstance(c, torch.nn.Conv2d)]
+    assert geo == ref["geo_resnet50dilated_ppm"]
+
+
+def test_east_decoder_reproduces_stored_reference_outputs():
+    """decoders/east.py:7-60 on CPU: the reference's parameters -> its loss, metrics and predictions (train and eval branches)."""
+    import megreader_b200.refapi.decoders as md
+    from oracle.make_ref_golden_cpu import east_case
+    g = np.load(os.path.join(GOLD, "east_ref.npz"))
+    m = md.EASTDecoder(channels=32).train()
+    m.load_state_dict({k[3:]: torch.from_numpy(g[k]) for k in g.files if k.startswith("sd.")})
+    x, label = east_case()
+    lm, pm, mm = m(x, label, None, True)
+    close = lambda a, k: torch.testing.assert_close(a.detach(), torch.from_numpy(g[k]), rtol=1e-4, atol=1e-5)  # noqa: E731
+    close(lm, "train.loss")
+    for k in pm:
+        close(pm[k], "train.pred." + k)
+    for k in mm:
+        close(mm[k], "train.metric." + k)
+    assert {"train.pred." + k for k in pm} | {"train.metric." + k for k in mm} == {k for k in g.files if k.startswith("train.") and k != "train.loss"}
+    m.eval()
+    pe = m(x, label, None, False)
+    for k in pe:
+        close(pe[k], "eval.pred." + k)
+
+
+@pytest.mark.skipif(not ref_loader.available(), reason="reference tree not present (the stored reference data above is compared anywhere)")
 def test_state_dict_keys_equal_reference():
     import sys
     import types
@@ -86,7 +154,7 @@ def test_state_dict_keys_equal_reference():
     assert geo(rp) == geo(mp)
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="/root/reference not present")
+@pytest.mark.skipif(not ref_loader.available(), reason="reference tree not present (the stored reference data above is compared anywhere)")
 def test_east_decoder_equals_reference_module():
     """decoders/east.py:7-60 on CPU: same parameters -> same loss, metrics and predictions (train and eval branches)."""
     ref_loader.install()

@@ -1,5 +1,5 @@
 """GPU: refapi surfaces around the hot path against the reference goldens (fp32, TF32 off), the 1-D CTC conv head through
-the sm_100a CTC kernels, and the deformable ResNet units through the sm_100a DCN kernels (checked against the CPU oracle
+the sm_90a CTC kernels, and the deformable ResNet units through the sm_90a DCN kernels (checked against the CPU oracle
 and against the closed form for zero offsets: modulated DCN with offset 0 and mask 1/2 == half a dense conv)."""
 import numpy as np
 import pytest

@@ -1,4 +1,4 @@
-"""GPU: the cfg-3 / cfg-4 models (BASELINE.json) with EVERY convolution on the repo's tcgen05 kernels (conv_engine) against the
+"""GPU: the cfg-3 / cfg-4 models (BASELINE.json) with EVERY convolution on the repo's wgmma kernels (conv_engine) against the
 same modules on the library path in fp32: training loss within bf16 tolerance, finite gradients for every parameter, and the
 parameter gradients' direction (cosine) for the layers that see the largest signals."""
 import pytest
