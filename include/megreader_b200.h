@@ -237,9 +237,11 @@ int mr_gemm_batched(const void *A, const void *B, void *C, int64_t M, int64_t N,
                     int in_dtype, int out_dtype, float alpha, float beta, void *stream);
 
 /* Hand-written Hopper GEMM (wgmma.mma_async with register accumulators + TMA operand staging), bf16 in / fp32 accumulate.
- * Same storage convention as mr_gemm; supported forms (transA,transB) = (0,1) and (1,0); optional per-column bias
- * and ReLU in the epilogue; beta = 1 accumulates atomically into fp32 C and enables split-K.  Returns
- * MR_ERR_UNSUPPORTED for shapes / alignments it does not cover (the caller then uses mr_gemm). */
+ * Same storage convention as mr_gemm; supported forms (transA,transB) = (0,1) "NT", (0,0) "NN" and (1,0) "TN"; optional
+ * per-column bias and ReLU in the epilogue; beta = 1 accumulates atomically into fp32 C and enables split-K.  The epilogue
+ * runs once per split, so bias with splits > 1 and ReLU with beta = 1 are refused (beta = 1, splits = 1 with bias gives
+ * C + AB + bias).  Returns MR_ERR_UNSUPPORTED for shapes / alignments / combinations it does not cover (the caller then
+ * uses mr_gemm). */
 int mr_gemm_tcgen05(const void *A, const void *B, void *C, int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb,
                     int64_t ldc, int transA, int transB, int out_dtype, const float *bias, int relu, float beta,
                     int splits, void *stream);

@@ -974,7 +974,7 @@ int mr_dcn_forward_fused_f32(const float *input, const float *weight, const floa
     rc = make_map(&tl, wlo, Kt, Cout, Kt, BK, 128);
     if (rc) return rc;
     /* two stages, not three: the 64 KB saved become L1 for the gathers (MR_DCN_STAGES3 selects three for experiments) */
-    static const bool three = getenv("MR_DCN_STAGES3") != nullptr;
+    const bool three = getenv("MR_DCN_STAGES3") != nullptr;
     if (three) return launch_dcn_fwd<128, 3>(th, tl, a, st);
     return launch_dcn_fwd<128, 2>(th, tl, a, st);
 }

@@ -823,7 +823,10 @@ extern "C" {
  * transB = 1: B stored [N,K] (ldb >= K);  transB = 0: B stored [K,N] (ldb >= N).   [same convention as mr_gemm]
  * Supported operand forms: (transA, transB) = (0, 1) "NT", (0, 0) "NN" and (1, 0) "TN".  lda, ldb multiples of 8, bases 16-byte
  * aligned.  out_dtype 0 = fp32, 1 = bf16.  beta must be 0 or 1; beta = 1 (fp32 only) accumulates atomically and allows
- * split-K (splits > 1).  Returns MR_ERR_UNSUPPORTED for anything else so that the caller can route to mr_gemm. */
+ * split-K (splits > 1).  Every split-K CTA runs the epilogue on its partial sum, so bias is refused when splits > 1 is
+ * requested (it would be added once per split) and ReLU is refused with beta = 1 (it would clamp partial sums, and
+ * relu(C + AB) is not what an accumulating caller wants either).  Returns MR_ERR_UNSUPPORTED for anything else so that
+ * the caller can route to mr_gemm. */
 int mr_gemm_tcgen05(const void *A, const void *B, void *C, int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb,
                     int64_t ldc, int transA, int transB, int out_dtype, const float *bias, int relu, float beta,
                     int splits, void *stream) {
@@ -834,6 +837,7 @@ int mr_gemm_tcgen05(const void *A, const void *B, void *C, int64_t M, int64_t N,
     if (!nt && !tn && !nn) return MR_ERR_UNSUPPORTED;
     if (lda % 8 || ldb % 8 || ((uintptr_t)A % 16) || ((uintptr_t)B % 16)) return MR_ERR_UNSUPPORTED;
     if (beta != 0.f && (beta != 1.f || out_dtype != 0)) return MR_ERR_UNSUPPORTED;
+    if ((bias && splits > 1) || (relu && beta == 1.f)) return MR_ERR_UNSUPPORTED;   /* the epilogue runs once per split */
     if (K == 0 || M > (1LL << 31) - 256 || N > (1LL << 31) - 256 || K > (1LL << 31) - 256) return MR_ERR_UNSUPPORTED;
     if (splits < 1) splits = 1;
     if (splits > 1 && beta != 1.f) return MR_ERR_UNSUPPORTED;
@@ -903,14 +907,14 @@ int mr_conv2d_fprop_tcgen05(const void *x, const void *Wm, void *y, int N, int H
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     /* TMA-A variant: tile the output space with boxes of 128 pixels, width cut into power-of-two segments. */
-    static const bool no_tma_a = getenv("MR_CONV_NO_TMA_A") != nullptr;
+    const bool no_tma_a = getenv("MR_CONV_NO_TMA_A") != nullptr;      /* read per call, like the other switches */
     a.nseg = 0;
     CUtensorMap tx[4];
     int tiles = 0;
     if (!no_tma_a) {
         int w0 = 0;
         bool ok = true;
-        while (w0 < a.Wo) {
+        while (ok && w0 < a.Wo) {                        /* ok = false: a box the TMA cannot take -> gather */
             if (a.nseg == 4) { ok = false; break; }
             int bw = 128;
             while (bw > a.Wo - w0) bw >>= 1;
@@ -935,7 +939,7 @@ int mr_conv2d_fprop_tcgen05(const void *x, const void *Wm, void *y, int N, int H
             for (int q = a.nseg; q < 4; ++q) tx[q] = tx[0];
             /* shallow rings leave room for 2-3 CTAs per SM, so one CTA's epilogue overlaps another's main loop
              * (the kernel is not persistent); MR_CONV_SHALLOW=0/1 overrides the default for experiments. */
-            static const char *sh_env = getenv("MR_CONV_SHALLOW");
+            const char *sh_env = getenv("MR_CONV_SHALLOW");
             const bool shallow = sh_env ? sh_env[0] == '1' : true;
             if (shallow) {
                 if (BN == 128) return launch_conv<128, 3, 1>(tb, tx, a, tiles, st);

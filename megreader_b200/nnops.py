@@ -226,8 +226,10 @@ def adam_step(p, g, m, v, lr, beta1, beta2, eps, step, grad_scale=1.0, shadow=No
 
 
 def gemm_tc(A, B, transA=False, transB=True, out=None, out_dtype=None, bias=None, relu=False, beta=0.0, splits=1):
-    """Hand-written wgmma/TMA bf16 GEMM (csrc/gemm_tcgen05.cu).  Same storage convention as gemm(); forms NT / TN.
-    Raises MegReaderB200Error(MR_ERR_UNSUPPORTED) for shapes it does not cover."""
+    """Hand-written wgmma/TMA bf16 GEMM (csrc/gemm_tcgen05.cu).  Same storage convention as gemm(); forms NT
+    (transA=False, transB=True), NN (False, False) and TN (True, False).  beta=1 accumulates into an fp32 `out` and allows
+    splits > 1; bias is refused with splits > 1 and relu with beta=1.  Raises MegReaderB200Error(MR_ERR_UNSUPPORTED) for
+    shapes and combinations it does not cover."""
     assert A.dim() == 2 and B.dim() == 2 and A.stride(1) == 1 and B.stride(1) == 1
     assert A.dtype == torch.bfloat16 and B.dtype == torch.bfloat16
     M, K = (A.size(1), A.size(0)) if transA else (A.size(0), A.size(1))

@@ -56,6 +56,17 @@ def test_argument_validation_without_gpu(so_path):
     assert rc == 3
     # empty batch is a no-op
     assert L.mr_ctc2d_forward_f32(None, None, None, None, 4, 2, 0, 5, 3, 3, 1, 0, 0, None, None, None) == 0
+    # wgmma GEMM: every split-K CTA runs the epilogue, so bias with splits > 1 and ReLU with beta = 1 are refused
+    # (aligned dummy pointers: the checks come before anything touches them)
+    A, B, C, bias = 0x10000, 0x20000, 0x30000, 0x40000
+    gemm = lambda transA, transB, bias, relu, beta, splits: L.mr_gemm_tcgen05(  # noqa: E731
+        A, B, C, 256, 256, 1024, 1024, 1024, 256, transA, transB, 0, bias, relu, beta, splits, None)
+    assert gemm(0, 1, bias, 0, 1.0, 2) == _lib.MR_ERR_UNSUPPORTED
+    assert gemm(1, 0, bias, 0, 1.0, 4) == _lib.MR_ERR_UNSUPPORTED
+    assert gemm(0, 1, None, 1, 1.0, 1) == _lib.MR_ERR_UNSUPPORTED
+    assert gemm(0, 0, bias, 1, 1.0, 1) == _lib.MR_ERR_UNSUPPORTED
+    assert gemm(1, 1, None, 0, 0.0, 1) == _lib.MR_ERR_UNSUPPORTED      # (transA, transB) = (1, 1)
+    assert gemm(0, 1, None, 0, 0.5, 1) == _lib.MR_ERR_UNSUPPORTED
 
 
 def test_product_never_imports_oracle():

@@ -5,6 +5,7 @@ import pytest
 import torch
 
 from oracle import capi
+from tests import wgmma_variants as wv
 
 pytestmark = pytest.mark.gpu
 
@@ -68,6 +69,21 @@ def test_dcn_forward_backward_vs_oracle(cuda, case):
         _close(tm.grad.cpu().numpy(), g_ref[4], "grad_mask")
     if with_bias:
         _close(tb.grad.cpu().numpy(), g_ref[2], "grad_bias")
+
+
+FUSED_FWD_CASE = 8      # stride 2, ragged tiles: the fused wgmma forward
+
+
+@pytest.mark.parametrize("stages3", [False, True], ids=["2stages", "3stages"])
+def test_dcn_fused_forward_rings(cuda, stages3, monkeypatch):
+    """the fused forward with its default two-stage ring and with MR_DCN_STAGES3=1 (read on every call)."""
+    monkeypatch.delenv("MR_DCN_STAGES3", raising=False)
+    if stages3:
+        monkeypatch.setenv("MR_DCN_STAGES3", "1")
+    wv.run_variant(wv.expected_variant("dcn_fwd"), lambda: test_dcn_forward_backward_vs_oracle(cuda, CASES[FUSED_FWD_CASE]))
+
+
+VARIANTS = {wv.expected_variant("dcn_fwd", env={}), wv.expected_variant("dcn_fwd", env={"MR_DCN_STAGES3": "1"})}
 
 
 def test_dcn_stride2_offset_slice_quirk(cuda):
