@@ -86,8 +86,15 @@ _SIGS = {
     "mr_dcn_wgrad_fused_f32": [c_p, c_p, c_i64, c_p, c_i64, c_p, c_p, c_f32, c_p, c_i64] + [c_int] * 15 + [c_p],
     "mr_dcn_backward_f32": [c_p, c_p, c_p, c_i64, c_p, c_i64, c_p, c_p, c_p, c_p, c_p, c_i64, c_p, c_i64, c_f32,
                             c_p, c_i64] + [c_int] * 15 + [c_p],
+    "mr_dcn_fused_workspace_bytes_h": [c_i64] * 7,
+    "mr_dcn_fused_backward_workspace_bytes_h": [c_i64] * 9,
+    "mr_dcn_forward_fused_h": [c_p, c_p, c_p, c_p, c_i64, c_p, c_i64, c_p, c_p, c_i64] + [c_int] * 17 + [c_p],
+    "mr_dcn_backward_fused_h": [c_p, c_p, c_p, c_i64, c_p, c_i64, c_p, c_p, c_p, c_p, c_p, c_i64, c_p, c_i64, c_f32,
+                                c_p, c_i64] + [c_int] * 17 + [c_p],
 }
 _RESTYPES = {
+    "mr_dcn_fused_workspace_bytes_h": c_i64,
+    "mr_dcn_fused_backward_workspace_bytes_h": c_i64,
     "mr_dcn_workspace_bytes": c_i64,
     "mr_dcn_fused_workspace_bytes": c_i64,
     "mr_dcn_fused_wgrad_workspace_bytes": c_i64,

@@ -22,6 +22,12 @@
 // Requirements of this path: group = 1, deformable_group = 1, C % 64 == 0, Cout % 128 == 0 (the ResNet-50 DCN units of
 // backbones/resnet.py:136-165 are C = Cout = 128 / 256 / 512); anything else uses the round-1 kernels in dcn.cu.
 // The offset / mask indexing quirk (flat (Ho,Wo) strides inside a possibly larger per-sample slab, SURVEY.md App. B2.1) is kept.
+//
+// Half precision (T = __half or bf16): the same three kernels, templated on the element type T of the input.  The NHWC copy,
+// the offsets, the mask, grad_output and the packed weights are T; sampling positions, the bilinear blend and the mask are
+// fp32 and each column value is rounded ONCE to T, so there is one operand (no hi / lo split) and one MMA per K block
+// (.f32.f16.f16 or .f32.bf16.bf16), still accumulated in fp32.  The fp32 kernels keep their names and code: their __global__
+// functions are thin wrappers around the T = float instantiation of the shared __device__ bodies.
 #include "wgmma.cuh"
 #include <math.h>
 #include <stdlib.h>
@@ -29,22 +35,62 @@
 
 namespace {
 
-struct DcnFArgs {
-    const float *xh;          // [B][H][W][C] fp32
-    const float *off, *msk;   // reference layout, per-sample slabs
+// ---------------------------------------------------------------- element type of the input (float, __half, bf16)
+template <typename T> struct DcnElem {                       // fp32 input: hi / lo bf16 split, three MMAs per K block
+    static constexpr bool kSplit = true;
+    static constexpr int kOps = 2;
+    typedef bf16 Mma;
+};
+template <> struct DcnElem<__half> { static constexpr bool kSplit = false; static constexpr int kOps = 1; typedef __half Mma; };
+template <> struct DcnElem<bf16> { static constexpr bool kSplit = false; static constexpr int kOps = 1; typedef bf16 Mma; };
+
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
+__device__ __forceinline__ float to_f32(bf16 v) { return __bfloat162float(v); }
+template <typename T> __device__ __forceinline__ T from_f32(float v);
+template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
+template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
+template <> __device__ __forceinline__ bf16 from_f32<bf16>(float v) { return __float2bfloat16_rn(v); }
+// one element / four consecutive elements through the read-only path, as fp32
+template <typename T> __device__ __forceinline__ float ld1(const T *p) { return to_f32(__ldg(p)); }
+__device__ __forceinline__ float4 ld4(const float *p) { return __ldg(reinterpret_cast<const float4 *>(p)); }
+template <typename T> __device__ __forceinline__ float4 ld4(const T *p) {
+    const uint2 u = __ldg(reinterpret_cast<const uint2 *>(p));
+    const T *h = reinterpret_cast<const T *>(&u);
+    return make_float4(to_f32(h[0]), to_f32(h[1]), to_f32(h[2]), to_f32(h[3]));
+}
+// channels [cb * 64 + e * 32, +4) of a pixel row of the NHWC copy (fp32: the float4 index arithmetic of the fp32 kernels)
+__device__ __forceinline__ float4 ld4_blk(const float *row, int cb, int e) { return __ldg(reinterpret_cast<const float4 *>(row) + cb * (BK / 4) + e * 8); }
+template <typename T> __device__ __forceinline__ float4 ld4_blk(const T *row, int cb, int e) { return ld4(row + cb * BK + e * 32); }
+// four fp32 -> four T in 8 bytes (round to nearest even)
+template <typename T> __device__ __forceinline__ uint2 pack4(float v0, float v1, float v2, float v3) {
+    uint2 r;
+    T *h = reinterpret_cast<T *>(&r);
+    h[0] = from_f32<T>(v0); h[1] = from_f32<T>(v1); h[2] = from_f32<T>(v2); h[3] = from_f32<T>(v3);
+    return r;
+}
+
+template <typename T> struct DcnFArgsT {
+    const T *xh;              // [B][H][W][C]
+    const T *off, *msk;       // reference layout, per-sample slabs
     const float *bias;
-    float *out;               // [B][Cout][Ho*Wo]
+    T *out;                   // [B][Cout][Ho*Wo]
     int64_t off_bs, mask_bs;
     int B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, Ho, Wo, P;
     int tiles_per_sample, tiles_x, ncb, nkb;     // 8 x 16 pixel tiles; ncb = C / 64 channel blocks, nkb = kh*kw*ncb K blocks
 };
+struct DcnFArgs : DcnFArgsT<float> {};
 
-template <int BN, int STAGES>
+// OPS = 2: fp32 input (hi and lo of both operands), 1: half precision
+template <int BN, int STAGES, int OPS = 2>
 struct DcnSmem {
     static constexpr int A_BYTES = BM * BK * 2;               // one of (hi, lo)
     static constexpr int B_BYTES = BN * BK * 2;
-    static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * B_BYTES;
-    static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+    static constexpr int STAGE_BYTES = OPS * A_BYTES + OPS * B_BYTES;
+    // the accumulator tile [128][BN + 1] fp32 is laid over the drained ring when the K loop is over, so the barriers and the tap
+    // table start behind whichever is larger (the fp32 ring of 128 / 192 KB always is; the 64 KB half-precision ring is not)
+    static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+    static constexpr int BAR_OFF = RING_BYTES >= AccTile<BN>::BYTES ? RING_BYTES : (AccTile<BN>::BYTES + 127) / 128 * 128;
     static constexpr int TAP_OFF = BAR_OFF + 128;             // barriers live in the first 128 bytes
     static constexpr int total(int taps) { return TAP_OFF + BM * taps * 24 + 1024; }   // + tap table (16 + 8 bytes / entry)
 };
@@ -57,10 +103,12 @@ __device__ __forceinline__ void mbar_arrive_cta(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
-template <int BN, int STAGES>
-__global__ void __launch_bounds__(kDcnThreads, 1)
-dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, DcnFArgs a) {
-    using L = DcnSmem<BN, STAGES>;
+// The forward body.  T = float: operands hi / lo from tmWh / tmWl, three MMAs per K block; T = __half / bf16: one operand
+// (tmWl is not read), one MMA per K block.
+template <typename T, int BN, int STAGES>
+__device__ __forceinline__ void dcn_fwd_body(const CUtensorMap &tmWh, const CUtensorMap &tmWl, const DcnFArgsT<T> &a) {
+    typedef DcnElem<T> X;
+    using L = DcnSmem<BN, STAGES, X::kOps>;
     extern __shared__ unsigned char smem_raw[];
     unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
@@ -79,19 +127,21 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmWh);
-        tma_prefetch_desc(&tmWl);
+        if constexpr (X::kSplit) tma_prefetch_desc(&tmWl);
         for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1 + kProducerThreads); mbar_init(empty + s, 1); }
         mbar_init(tmem_full, 1);
         fence_barrier_init();
     }
     __syncthreads();
     float *acc_tile = (float *)smem;                         // laid over the drained operand ring when the K loop is over
+    static_assert(L::BAR_OFF >= AccTile<BN>::BYTES, "the accumulator tile must end before the barriers");
 
     // 768 threads leave 80 registers each: the MMA warpgroup takes what its 128 accumulator registers need from the others
     if (threadIdx.x >= kDcnMma0) {
         reg_inc<160>();
-        // ------------------------------------------------------------ MMA warpgroup: D += Ah Wh + Ah Wl + Al Wh
+        // ------------------------------------------------------------ MMA warpgroup: D += Ah Wh + Ah Wl + Al Wh (fp32) / A W (T)
         static_assert(BN == 128, "one warpgroup holds a 128 x 128 accumulator");
+        constexpr int PASSES = X::kSplit ? 3 : 1;
         const int mt = threadIdx.x - kDcnMma0;
         AccTile<BN> acc;
         uint64_t *pending = nullptr;
@@ -100,17 +150,17 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
             mbar_wait(full + s, (i / STAGES) & 1);
             const uint32_t ah = smem_u32(smem + s * L::STAGE_BYTES);
             const uint32_t al = ah + L::A_BYTES;
-            const uint32_t bh = al + L::A_BYTES;
+            const uint32_t bh = ah + X::kOps * L::A_BYTES;
             const uint32_t bl = bh + L::B_BYTES;
             wgmma_fence();
 #pragma unroll
-            for (int pass = 0; pass < 3; ++pass) {
+            for (int pass = 0; pass < PASSES; ++pass) {
                 const uint32_t aa = pass == 2 ? al : ah, bb = pass == 1 ? bl : bh;
 #pragma unroll
                 for (int k = 0; k < BK / UMMA_K; ++k)
-                    acc.template mma_halves<0, 0>(make_desc(aa + k * 32, 16, 1024), make_desc(aa + 64 * 128 + k * 32, 16, 1024),
-                                                  make_desc(bb + k * 32, 16, 1024), make_desc(bb + 64 * 128 + k * 32, 16, 1024),
-                                                  (i | pass | k) != 0);
+                    acc.template mma_halves<0, 0, typename X::Mma>(make_desc(aa + k * 32, 16, 1024), make_desc(aa + 64 * 128 + k * 32, 16, 1024),
+                                                                   make_desc(bb + k * 32, 16, 1024), make_desc(bb + 64 * 128 + k * 32, 16, 1024),
+                                                                   (i | pass | k) != 0);
             }
             wgmma_commit();
             wgmma_wait<1>();
@@ -132,10 +182,10 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
             for (int i = 0; i < nkb; ++i) {
                 const int s = i % STAGES;
                 mbar_wait(empty + s, ((i / STAGES) & 1) ^ 1);
-                unsigned char *st = smem + s * L::STAGE_BYTES + 2 * L::A_BYTES;
-                mbar_expect_tx(full + s, 2 * L::B_BYTES);
+                unsigned char *st = smem + s * L::STAGE_BYTES + X::kOps * L::A_BYTES;
+                mbar_expect_tx(full + s, X::kOps * L::B_BYTES);
                 tma_load_2d(&tmWh, full + s, st, i * BK, n0);
-                tma_load_2d(&tmWl, full + s, st + L::B_BYTES, i * BK, n0);
+                if constexpr (X::kSplit) tma_load_2d(&tmWl, full + s, st + L::B_BYTES, i * BK, n0);
             }
         }
     } else if (warp >= 2 && threadIdx.x < 64 + kProducerThreads) {
@@ -146,15 +196,15 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
         // the gathers were bound by the L1 data stage.
         const int pwp = warp - 2;                             // producer warp 0..15
         const int sub = lane >> 3, j = lane & 7;
-        struct Row { const float4 *q1, *q2, *q3, *q4; float w1, w2, w3, w4; };
-        const float *xb = a.xh + (int64_t)b * a.H * a.W * a.C + j * 4;
+        struct Row { const T *q1, *q2, *q3, *q4; float w1, w2, w3, w4; };
+        const T *xb = a.xh + (int64_t)b * a.H * a.W * a.C + j * 4;
         // ---- tap table: the bilinear set-up of every (row, tap) of this tile is computed ONCE (one entry per producer thread
         // and pass) instead of by each of the 8 lanes that share a row: 4 weights (mask and validity folded in) + 4 clamped
         // corner coordinates (uint16), 24 bytes per entry.
         {
             const int nent = BM * a.kh * a.kw;
-            const float *offb = a.off + (int64_t)b * a.off_bs;
-            const float *mskb = a.msk ? a.msk + (int64_t)b * a.mask_bs : nullptr;
+            const T *offb = a.off + (int64_t)b * a.off_bs;
+            const T *mskb = a.msk ? a.msk + (int64_t)b * a.mask_bs : nullptr;
             for (int e = threadIdx.x - 64; e < nent; e += kProducerThreads) {
                 const int k = e / BM, r = e - k * BM;
                 const int py = ty0 + (r >> 4), px = tx0 + (r & 15);
@@ -162,9 +212,9 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
                 const int ho = rok ? py : a.Ho - 1, wo = rok ? px : a.Wo - 1;
                 const int pc = ho * a.Wo + wo;
                 const int ti = k / a.kw, tj = k - ti * a.kw;
-                const float oh = __ldg(offb + (int64_t)(2 * k) * a.P + pc);
-                const float ow = __ldg(offb + (int64_t)(2 * k + 1) * a.P + pc);
-                const float m = mskb ? __ldg(mskb + (int64_t)k * a.P + pc) : 1.f;
+                const float oh = ld1(offb + (int64_t)(2 * k) * a.P + pc);
+                const float ow = ld1(offb + (int64_t)(2 * k + 1) * a.P + pc);
+                const float m = mskb ? ld1(mskb + (int64_t)k * a.P + pc) : 1.f;
                 const float hy = (float)(ho * a.sh - a.ph + ti * a.dh) + oh;
                 const float wx = (float)(wo * a.sw - a.pw + tj * a.dw) + ow;
                 // dmcn_im2col_bilinear (deform_conv_cuda_kernel.cu:466-496): zero outside (-1,H) x (-1,W), corners outside dropped
@@ -197,21 +247,20 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
                 rw[u].w1 = wv.x; rw[u].w2 = wv.y; rw[u].w3 = wv.z; rw[u].w4 = wv.w;
                 const int y0 = (int)(cv.x & 0xffffu) * a.W, y1 = (int)(cv.x >> 16) * a.W;
                 const int x0 = (int)(cv.y & 0xffffu), x1 = (int)(cv.y >> 16);
-                rw[u].q1 = reinterpret_cast<const float4 *>(xb + (int64_t)(y0 + x0) * a.C);
-                rw[u].q2 = reinterpret_cast<const float4 *>(xb + (int64_t)(y0 + x1) * a.C);
-                rw[u].q3 = reinterpret_cast<const float4 *>(xb + (int64_t)(y1 + x0) * a.C);
-                rw[u].q4 = reinterpret_cast<const float4 *>(xb + (int64_t)(y1 + x1) * a.C);
+                rw[u].q1 = xb + (int64_t)(y0 + x0) * a.C;
+                rw[u].q2 = xb + (int64_t)(y0 + x1) * a.C;
+                rw[u].q3 = xb + (int64_t)(y1 + x0) * a.C;
+                rw[u].q4 = xb + (int64_t)(y1 + x1) * a.C;
             }
             {
                 // all 16 gathers of this thread are issued before the slot wait and before any use
                 float4 x1[2][2], x2[2][2], x3[2][2], x4[2][2];
-                const int c4 = cc * (BK / 4);
 #pragma unroll
                 for (int u = 0; u < 2; ++u)
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
-                        x1[u][e] = __ldg(rw[u].q1 + c4 + e * 8); x2[u][e] = __ldg(rw[u].q2 + c4 + e * 8);
-                        x3[u][e] = __ldg(rw[u].q3 + c4 + e * 8); x4[u][e] = __ldg(rw[u].q4 + c4 + e * 8);
+                        x1[u][e] = ld4_blk(rw[u].q1, cc, e); x2[u][e] = ld4_blk(rw[u].q2, cc, e);
+                        x3[u][e] = ld4_blk(rw[u].q3, cc, e); x4[u][e] = ld4_blk(rw[u].q4, cc, e);
                     }
                 const int s = kb % STAGES;
                 mbar_wait(empty + s, ((kb / STAGES) & 1) ^ 1);
@@ -225,18 +274,23 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
                         const float v1 = rw[u].w1 * x1[u][e].y + rw[u].w2 * x2[u][e].y + rw[u].w3 * x3[u][e].y + rw[u].w4 * x4[u][e].y;
                         const float v2 = rw[u].w1 * x1[u][e].z + rw[u].w2 * x2[u][e].z + rw[u].w3 * x3[u][e].z + rw[u].w4 * x4[u][e].z;
                         const float v3 = rw[u].w1 * x1[u][e].w + rw[u].w2 * x2[u][e].w + rw[u].w3 * x3[u][e].w + rw[u].w4 * x4[u][e].w;
-                        uint2 hi, lo;
-                        __nv_bfloat162 *h2 = reinterpret_cast<__nv_bfloat162 *>(&hi);
-                        __nv_bfloat162 *l2 = reinterpret_cast<__nv_bfloat162 *>(&lo);
-                        h2[0] = __floats2bfloat162_rn(v0, v1);
-                        h2[1] = __floats2bfloat162_rn(v2, v3);
-                        const float2 f0 = __bfloat1622float2(h2[0]), f1 = __bfloat1622float2(h2[1]);
-                        l2[0] = __floats2bfloat162_rn(v0 - f0.x, v1 - f0.y);
-                        l2[1] = __floats2bfloat162_rn(v2 - f1.x, v3 - f1.y);
                         // channels e*32 + 4j .. +3 -> 16-byte chunk e*4 + j/2 of the row (swizzled), 8-byte half j & 1
                         const uint32_t o = row_off + ((((uint32_t)(e * 4 + (j >> 1))) ^ sw) << 4) + (uint32_t)(j & 1) * 8u;
-                        asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(ah_s + o), "r"(hi.x), "r"(hi.y) : "memory");
-                        asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(ah_s + (uint32_t)L::A_BYTES + o), "r"(lo.x), "r"(lo.y) : "memory");
+                        if constexpr (X::kSplit) {
+                            uint2 hi, lo;
+                            __nv_bfloat162 *h2 = reinterpret_cast<__nv_bfloat162 *>(&hi);
+                            __nv_bfloat162 *l2 = reinterpret_cast<__nv_bfloat162 *>(&lo);
+                            h2[0] = __floats2bfloat162_rn(v0, v1);
+                            h2[1] = __floats2bfloat162_rn(v2, v3);
+                            const float2 f0 = __bfloat1622float2(h2[0]), f1 = __bfloat1622float2(h2[1]);
+                            l2[0] = __floats2bfloat162_rn(v0 - f0.x, v1 - f0.y);
+                            l2[1] = __floats2bfloat162_rn(v2 - f1.x, v3 - f1.y);
+                            asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(ah_s + o), "r"(hi.x), "r"(hi.y) : "memory");
+                            asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(ah_s + (uint32_t)L::A_BYTES + o), "r"(lo.x), "r"(lo.y) : "memory");
+                        } else {
+                            const uint2 h = pack4<T>(v0, v1, v2, v3);          // the one rounding of the column value
+                            asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(ah_s + o), "r"(h.x), "r"(h.y) : "memory");
+                        }
                     }
                 }
                 fence_proxy_async();                          // generic-proxy smem writes -> visible to wgmma
@@ -250,7 +304,7 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
         const int ey = ty0 + (er >> 4), ex = tx0 + (er & 15);
         const int prow = (ey < a.Ho && ex < a.Wo) ? ey * a.Wo + ex : a.P;
         mbar_wait(tmem_full, 0);
-        float *ob = a.out + ((int64_t)b * a.Cout + n0) * a.P + prow;
+        T *ob = a.out + ((int64_t)b * a.Cout + n0) * a.P + prow;
 #pragma unroll 1
         for (int c = part * (BN / 128); c < (part + 1) * (BN / 128); ++c) {
             uint32_t rr[32];
@@ -261,11 +315,24 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
                     const int co = c * 32 + j;
                     float v = __uint_as_float(rr[j]);
                     if (a.bias) v += __ldg(a.bias + n0 + co);
-                    ob[(int64_t)co * a.P] = v;
+                    ob[(int64_t)co * a.P] = from_f32<T>(v);
                 }
             }
         }
     }
+}
+
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(kDcnThreads, 1)
+dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, DcnFArgs a) {
+    dcn_fwd_body<float, BN, STAGES>(tmWh, tmWl, a);
+}
+
+// half-precision forward: T = __half or bf16, two-stage ring (32 KB per stage), output T
+template <typename T>
+__global__ void __launch_bounds__(kDcnThreads, 1)
+dcn_fwd_half_kernel(const __grid_constant__ CUtensorMap tmW, DcnFArgsT<T> a) {
+    dcn_fwd_body<T, 128, 2>(tmW, tmW, a);
 }
 
 // =====================================================================================================
@@ -277,28 +344,33 @@ dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_co
 // of the pixel tiles (split-K); the A operand is grad_output re-tiled to [b * tiles + tile][co][128 pixels in tile order] and split
 // into bf16 hi / lo by a small pre-pass, so that one pixel tile of it is a plain 2-D TMA box.  fp32 atomics at the end.
 // =====================================================================================================
-struct DcnWArgs {
-    const float *xh, *off, *msk;
+// (half precision: grad_output re-tiled to ONE T copy, single-operand column tiles, one MMA per pixel tile; the atomics stay fp32)
+template <typename T> struct DcnWArgsT {
+    const T *xh, *off, *msk;
     float *gw;                // [Cout][C][kh*kw] fp32, accumulated
     int64_t off_bs, mask_bs;
     float scale;
     int B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, Ho, Wo, P;
     int tiles_per_sample, tiles_x, ncb, nkb, ntiles, splits;
 };
+struct DcnWArgs : DcnWArgsT<float> {};
 
-struct DcnWSmem {
+template <int OPS>
+struct DcnWSmemT {
     static constexpr int B_BYTES = BM * BK * 2;               // produced tile, one of (hi, lo): [128 pixels][64 kc]
     static constexpr int A_BYTES = BM * BM * 2;               // go tile, one of (hi, lo): [128 co][128 pixels] = two 64-pixel atoms
     static constexpr int STAGES = 2;                          // of the produced operand; the TMA operand has ONE buffer: its load for tile
-    static constexpr int A_OFF = STAGES * 2 * B_BYTES;        // i + 1 is issued when the MMAs of tile i retire and lands while tile i + 1
-    static constexpr int BAR_OFF = A_OFF + 2 * A_BYTES;       // is being gathered -- 64 KB less shared memory = 64 KB more L1 for the gathers
+    static constexpr int A_OFF = STAGES * OPS * B_BYTES;      // i + 1 is issued when the MMAs of tile i retire and lands while tile i + 1
+    static constexpr int BAR_OFF = A_OFF + OPS * A_BYTES;     // is being gathered -- 64 KB less shared memory = 64 KB more L1 for the gathers
     static constexpr int TAP_OFF = BAR_OFF + 128;
     static constexpr int TOTAL = TAP_OFF + 2 * BM * 24 + 1024;   // one tap-table row set per tile parity
 };
+typedef DcnWSmemT<2> DcnWSmem;
 
-__global__ void __launch_bounds__(kDcnThreads, 1)
-dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_constant__ CUtensorMap tmGl, DcnWArgs a) {
-    using L = DcnWSmem;
+template <typename T>
+__device__ __forceinline__ void dcn_wgrad_body(const CUtensorMap &tmGh, const CUtensorMap &tmGl, const DcnWArgsT<T> &a) {
+    typedef DcnElem<T> X;
+    using L = DcnWSmemT<X::kOps>;
     constexpr int STAGES = L::STAGES;
     extern __shared__ unsigned char smem_raw[];
     unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -317,7 +389,7 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&tmGh);
-        tma_prefetch_desc(&tmGl);
+        if constexpr (X::kSplit) tma_prefetch_desc(&tmGl);
         for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, kProducerThreads); mbar_init(empty + s, 1); }
         mbar_init(a_full, 1); mbar_init(a_empty, 1);
         mbar_init(tmem_full, 1);
@@ -325,6 +397,7 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
     }
     __syncthreads();
     float *acc_tile = (float *)smem;                         // laid over the drained operand ring when the loop is over
+    static_assert(L::BAR_OFF >= AccTile<BN>::BYTES, "the accumulator tile must end before the barriers");
 
     if (warp == 0) {
         if (elect_one()) {
@@ -332,35 +405,38 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                 const int gt = (int)blockIdx.y + i * a.splits;
                 mbar_wait(a_empty, (i & 1) ^ 1);
                 unsigned char *st = smem + L::A_OFF;
-                mbar_expect_tx(a_full, 2 * L::A_BYTES);
+                mbar_expect_tx(a_full, X::kOps * L::A_BYTES);
                 const int row = gt * a.Cout + co0;                        // rows of the re-tiled grad_output: (tile, co)
                 tma_load_2d(&tmGh, a_full, st, 0, row);
                 tma_load_2d(&tmGh, a_full, st + BM * 128, 64, row);
-                tma_load_2d(&tmGl, a_full, st + L::A_BYTES, 0, row);
-                tma_load_2d(&tmGl, a_full, st + L::A_BYTES + BM * 128, 64, row);
+                if constexpr (X::kSplit) {
+                    tma_load_2d(&tmGl, a_full, st + L::A_BYTES, 0, row);
+                    tma_load_2d(&tmGl, a_full, st + L::A_BYTES + BM * 128, 64, row);
+                }
             }
         }
     } else if (threadIdx.x >= kDcnMma0) {
         // A K-major (pixels contiguous), B MN-major (kc contiguous)
+        constexpr int PASSES = X::kSplit ? 3 : 1;
         const int mt = threadIdx.x - kDcnMma0;
         AccTile<BN> acc;
         for (int i = 0; i < nt; ++i) {
             const int s = i % STAGES;
             mbar_wait(full + s, (i / STAGES) & 1);
             mbar_wait(a_full, i & 1);
-            const uint32_t bh = smem_u32(smem + s * 2 * L::B_BYTES);
+            const uint32_t bh = smem_u32(smem + s * X::kOps * L::B_BYTES);
             const uint32_t bl = bh + L::B_BYTES;
             const uint32_t ah = smem_u32(smem + L::A_OFF);
             const uint32_t al = ah + L::A_BYTES;
             wgmma_fence();
 #pragma unroll
-            for (int pass = 0; pass < 3; ++pass) {
+            for (int pass = 0; pass < PASSES; ++pass) {
                 const uint32_t aa = pass == 2 ? al : ah, bb = pass == 1 ? bl : bh;       // Ah Bh, Ah Bl, Al Bh
 #pragma unroll
                 for (int j = 0; j < BM / UMMA_K; ++j) {                                   // 8 steps of 16 pixels
                     const uint32_t ak = aa + (j >> 2) * (BM * 128) + (j & 3) * 32;
-                    acc.mma<0, 1>(make_desc(ak, 16, 1024), make_desc(ak + 64 * 128, 16, 1024), make_desc(bb + j * 2048, BM * 128, 1024),
-                                  (i | pass | j) != 0);
+                    acc.template mma<0, 1, typename X::Mma>(make_desc(ak, 16, 1024), make_desc(ak + 64 * 128, 16, 1024),
+                                                            make_desc(bb + j * 2048, BM * 128, 1024), (i | pass | j) != 0);
                 }
             }
             wgmma_commit();
@@ -389,10 +465,10 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
             const int py = (tile / a.tiles_x) * 8 + (r >> 4), px = (tile % a.tiles_x) * 16 + (r & 15);
             const bool rok = py < a.Ho && px < a.Wo;
             const int pc = (rok ? py : a.Ho - 1) * a.Wo + (rok ? px : a.Wo - 1);
-            const float *offb = a.off + (int64_t)bb * a.off_bs;
-            oh = __ldg(offb + (int64_t)(2 * k) * a.P + pc);
-            ow = __ldg(offb + (int64_t)(2 * k + 1) * a.P + pc);
-            m = a.msk ? __ldg(a.msk + (int64_t)bb * a.mask_bs + (int64_t)k * a.P + pc) : 1.f;
+            const T *offb = a.off + (int64_t)bb * a.off_bs;
+            oh = ld1(offb + (int64_t)(2 * k) * a.P + pc);
+            ow = ld1(offb + (int64_t)(2 * k + 1) * a.P + pc);
+            m = a.msk ? ld1(a.msk + (int64_t)bb * a.mask_bs + (int64_t)k * a.P + pc) : 1.f;
         };
         auto tap_store = [&](int gt, int slot, float oh, float ow, float m) {
             const int bb = gt / a.tiles_per_sample, tile = gt - bb * a.tiles_per_sample;
@@ -429,8 +505,7 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
             float noh = 0.f, now = 0.f, nm = 0.f;
             if (prep) tap_load(gt + a.splits, noh, now, nm);
             mbar_wait(empty + s, ((i / STAGES) & 1) ^ 1);
-            const float *xb = a.xh + (int64_t)b * a.H * a.W * a.C + j * 4;
-            const int c4 = cc * (BK / 4);
+            const T *xb = a.xh + (int64_t)b * a.H * a.W * a.C + j * 4;
             float4 x1[2][2], x2[2][2], x3[2][2], x4[2][2];
             float4 wv[2];
 #pragma unroll
@@ -439,17 +514,17 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                 const uint2 cv = tapc[rrow[u]];
                 const int y0 = (int)(cv.x & 0xffffu) * a.W, y1 = (int)(cv.x >> 16) * a.W;
                 const int x0 = (int)(cv.y & 0xffffu), xx1 = (int)(cv.y >> 16);
-                const float4 *q1 = reinterpret_cast<const float4 *>(xb + (int64_t)(y0 + x0) * a.C);
-                const float4 *q2 = reinterpret_cast<const float4 *>(xb + (int64_t)(y0 + xx1) * a.C);
-                const float4 *q3 = reinterpret_cast<const float4 *>(xb + (int64_t)(y1 + x0) * a.C);
-                const float4 *q4 = reinterpret_cast<const float4 *>(xb + (int64_t)(y1 + xx1) * a.C);
+                const T *q1 = xb + (int64_t)(y0 + x0) * a.C;
+                const T *q2 = xb + (int64_t)(y0 + xx1) * a.C;
+                const T *q3 = xb + (int64_t)(y1 + x0) * a.C;
+                const T *q4 = xb + (int64_t)(y1 + xx1) * a.C;
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    x1[u][e] = __ldg(q1 + c4 + e * 8); x2[u][e] = __ldg(q2 + c4 + e * 8);
-                    x3[u][e] = __ldg(q3 + c4 + e * 8); x4[u][e] = __ldg(q4 + c4 + e * 8);
+                    x1[u][e] = ld4_blk(q1, cc, e); x2[u][e] = ld4_blk(q2, cc, e);
+                    x3[u][e] = ld4_blk(q3, cc, e); x4[u][e] = ld4_blk(q4, cc, e);
                 }
             }
-            const uint32_t bh_s = smem_u32(smem + s * 2 * L::B_BYTES);
+            const uint32_t bh_s = smem_u32(smem + s * X::kOps * L::B_BYTES);
 #pragma unroll
             for (int u = 0; u < 2; ++u) {
                 const uint32_t row_off = (uint32_t)rrow[u] * 128u, sw = (uint32_t)(rrow[u] & 7);
@@ -459,17 +534,22 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                     const float v1 = wv[u].x * x1[u][e].y + wv[u].y * x2[u][e].y + wv[u].z * x3[u][e].y + wv[u].w * x4[u][e].y;
                     const float v2 = wv[u].x * x1[u][e].z + wv[u].y * x2[u][e].z + wv[u].z * x3[u][e].z + wv[u].w * x4[u][e].z;
                     const float v3 = wv[u].x * x1[u][e].w + wv[u].y * x2[u][e].w + wv[u].z * x3[u][e].w + wv[u].w * x4[u][e].w;
-                    uint2 hi, lo;
-                    __nv_bfloat162 *h2 = reinterpret_cast<__nv_bfloat162 *>(&hi);
-                    __nv_bfloat162 *l2 = reinterpret_cast<__nv_bfloat162 *>(&lo);
-                    h2[0] = __floats2bfloat162_rn(v0, v1);
-                    h2[1] = __floats2bfloat162_rn(v2, v3);
-                    const float2 f0 = __bfloat1622float2(h2[0]), f1 = __bfloat1622float2(h2[1]);
-                    l2[0] = __floats2bfloat162_rn(v0 - f0.x, v1 - f0.y);
-                    l2[1] = __floats2bfloat162_rn(v2 - f1.x, v3 - f1.y);
                     const uint32_t o = row_off + ((((uint32_t)(e * 4 + (j >> 1))) ^ sw) << 4) + (uint32_t)(j & 1) * 8u;
-                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(bh_s + o), "r"(hi.x), "r"(hi.y) : "memory");
-                    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(bh_s + (uint32_t)L::B_BYTES + o), "r"(lo.x), "r"(lo.y) : "memory");
+                    if constexpr (X::kSplit) {
+                        uint2 hi, lo;
+                        __nv_bfloat162 *h2 = reinterpret_cast<__nv_bfloat162 *>(&hi);
+                        __nv_bfloat162 *l2 = reinterpret_cast<__nv_bfloat162 *>(&lo);
+                        h2[0] = __floats2bfloat162_rn(v0, v1);
+                        h2[1] = __floats2bfloat162_rn(v2, v3);
+                        const float2 f0 = __bfloat1622float2(h2[0]), f1 = __bfloat1622float2(h2[1]);
+                        l2[0] = __floats2bfloat162_rn(v0 - f0.x, v1 - f0.y);
+                        l2[1] = __floats2bfloat162_rn(v2 - f1.x, v3 - f1.y);
+                        asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(bh_s + o), "r"(hi.x), "r"(hi.y) : "memory");
+                        asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(bh_s + (uint32_t)L::B_BYTES + o), "r"(lo.x), "r"(lo.y) : "memory");
+                    } else {
+                        const uint2 h = pack4<T>(v0, v1, v2, v3);
+                        asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(bh_s + o), "r"(h.x), "r"(h.y) : "memory");
+                    }
                 }
             }
             fence_proxy_async();
@@ -493,6 +573,17 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
     }
 }
 
+__global__ void __launch_bounds__(kDcnThreads, 1)
+dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_constant__ CUtensorMap tmGl, DcnWArgs a) {
+    dcn_wgrad_body<float>(tmGh, tmGl, a);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kDcnThreads, 1)
+dcn_wgrad_half_kernel(const __grid_constant__ CUtensorMap tmG, DcnWArgsT<T> a) {
+    dcn_wgrad_body<T>(tmG, tmG, a);
+}
+
 // =====================================================================================================
 // Fused DATA GRADIENT (round 2): grad_input, grad_offset, grad_mask without the column-gradient matrix
 //   colg[b, p, (k, c)] = sum_co go[b, co, p] * W[co, c, k]          (deform_conv_cuda.cpp:611-614, an SGEMM per sample in the reference)
@@ -506,20 +597,24 @@ dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
 // (128 contiguous bytes per 8 lanes), form the three per-pixel sums and scatter into an NHWC fp32 copy of grad_input with 16-byte
 // vector reductions (red.global.add.v4.f32), which a transpose-add folds into the caller's NCHW tensor.
 // =====================================================================================================
-struct DcnDArgs {
-    const float *xh, *off, *msk;
+// (half precision: one operand each, one MMA per K block; the corner gathers read the T NHWC copy, grad_input is still scattered
+// into the fp32 NHWC scratch, grad_offset / grad_mask are written in T)
+template <typename T> struct DcnDArgsT {
+    const T *xh, *off, *msk;
     float *gxh;                // [B][H][W][C] fp32, zero-filled; nullptr = no grad_input wanted
-    float *goff, *gmask;       // reference layouts (flat (Ho, Wo) strides inside per-sample slabs); either may be nullptr
+    T *goff, *gmask;           // reference layouts (flat (Ho, Wo) strides inside per-sample slabs); either may be nullptr
     int64_t off_bs, mask_bs, goff_bs, gmask_bs;
     int B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, Ho, Wo, P;
     int tiles_per_sample, tiles_x, nch, nkk, tap_splits;     // nch = C / 128 channel chunks, nkk = Cout / 32 K blocks
 };
+struct DcnDArgs : DcnDArgsT<float> {};
 
-struct DcnDSmem {
+template <int OPS>
+struct DcnDSmemT {
     static constexpr int BN = 128;
     static constexpr int KB = 32;                             // output channels (the reduction dimension) per pipeline stage
     static constexpr int OP_BYTES = KB * 128 * 2;             // one operand tile, one of (hi, lo): [32 co][128 (pixels | kc)] = 8 KB
-    static constexpr int STAGE_BYTES = 4 * OP_BYTES;          // A hi, A lo, B hi, B lo
+    static constexpr int STAGE_BYTES = 2 * OPS * OP_BYTES;    // A hi, A lo, B hi, B lo (A, B in half precision)
     static constexpr int STAGES = 2;                          // small on purpose: the epilogue's gathers want the rest of the SM's L1
     static constexpr int STG_OFF = STAGES * STAGE_BYTES;      // fp32 staging tile [128 pixels][128 channels], 16-byte chunks XOR-swizzled
     static constexpr int STG_BYTES = BM * BN * 4;
@@ -529,6 +624,7 @@ struct DcnDSmem {
     static constexpr int TAB_BYTES = 2 * BM * (3 * 16 + 8 + 4);          // tap tables, double-buffered by tap parity
     static constexpr int TOTAL = TAB_OFF + TAB_BYTES + 1024;
 };
+typedef DcnDSmemT<2> DcnDSmem;
 
 __device__ __forceinline__ void red_add_v4(float *p, float a, float b, float c, float d) {
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
@@ -542,18 +638,20 @@ struct DcnDTab {
     float *m;               // modulation mask
 };
 struct DcnDRaw { float oh, ow, m; };
-__device__ __forceinline__ DcnDRaw dcn_dgrad_load_row(const DcnDArgs &a, int b, int kk, int r, int ty0, int tx0) {
+template <typename T>
+__device__ __forceinline__ DcnDRaw dcn_dgrad_load_row(const DcnDArgsT<T> &a, int b, int kk, int r, int ty0, int tx0) {
     const int py = ty0 + (r >> 4), px = tx0 + (r & 15);
     const bool rok = py < a.Ho && px < a.Wo;
     const int pc = (rok ? py : a.Ho - 1) * a.Wo + (rok ? px : a.Wo - 1);
-    const float *offb = a.off + (int64_t)b * a.off_bs;
+    const T *offb = a.off + (int64_t)b * a.off_bs;
     DcnDRaw v;
-    v.oh = __ldg(offb + (int64_t)(2 * kk) * a.P + pc);
-    v.ow = __ldg(offb + (int64_t)(2 * kk + 1) * a.P + pc);
-    v.m = a.msk ? __ldg(a.msk + (int64_t)b * a.mask_bs + (int64_t)kk * a.P + pc) : 1.f;
+    v.oh = ld1(offb + (int64_t)(2 * kk) * a.P + pc);
+    v.ow = ld1(offb + (int64_t)(2 * kk + 1) * a.P + pc);
+    v.m = a.msk ? ld1(a.msk + (int64_t)b * a.mask_bs + (int64_t)kk * a.P + pc) : 1.f;
     return v;
 }
-__device__ __forceinline__ void dcn_dgrad_store_row(const DcnDArgs &a, const DcnDTab &t, const DcnDRaw &v, int kk, int r, int ty0, int tx0) {
+template <typename T>
+__device__ __forceinline__ void dcn_dgrad_store_row(const DcnDArgsT<T> &a, const DcnDTab &t, const DcnDRaw &v, int kk, int r, int ty0, int tx0) {
     const int ti = kk / a.kw, tj = kk - ti * a.kw;
     const int py = ty0 + (r >> 4), px = tx0 + (r & 15);
     const bool rok = py < a.Ho && px < a.Wo;
@@ -576,10 +674,11 @@ __device__ __forceinline__ void dcn_dgrad_store_row(const DcnDArgs &a, const Dcn
     t.m[r] = m;
 }
 
-__global__ void __launch_bounds__(kDcnThreads, 1)
-dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_constant__ CUtensorMap tmGl,
-                         const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, DcnDArgs a) {
-    using L = DcnDSmem;
+template <typename T>
+__device__ __forceinline__ void dcn_dgrad_body(const CUtensorMap &tmGh, const CUtensorMap &tmGl, const CUtensorMap &tmWh,
+                                               const CUtensorMap &tmWl, const DcnDArgsT<T> &a) {
+    typedef DcnElem<T> X;
+    using L = DcnDSmemT<X::kOps>;
     constexpr int STAGES = L::STAGES;
     constexpr int BN = L::BN;
     extern __shared__ unsigned char smem_raw[];
@@ -603,7 +702,10 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
     const int K = a.kh * a.kw;
 
     if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmGh); tma_prefetch_desc(&tmGl); tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
+        tma_prefetch_desc(&tmGh);
+        if constexpr (X::kSplit) tma_prefetch_desc(&tmGl);
+        tma_prefetch_desc(&tmWh);
+        if constexpr (X::kSplit) tma_prefetch_desc(&tmWl);
         for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); }
         for (int s = 0; s < 2; ++s) { mbar_init(acc_full + s, 1); mbar_init(acc_empty + s, kProducerThreads / 32); }
         fence_barrier_init();
@@ -616,6 +718,7 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
         reg_inc<160>();
         // both operands MN-major.  The accumulator of block n lives in registers, so its MMAs overlap the epilogue of block
         // n - 1; only the publication into the single shared tile waits until the epilogue warps have drained that block.
+        constexpr int PASSES = X::kSplit ? 3 : 1;
         const int mt = threadIdx.x - kDcnMma0;
         AccTile<BN> acc;
         int i = 0, n = 0;
@@ -627,16 +730,17 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                     const int s = i % STAGES;
                     mbar_wait(full + s, (i / STAGES) & 1);
                     const uint32_t ah = smem_u32(smem + s * L::STAGE_BYTES);
-                    const uint32_t al = ah + L::OP_BYTES, bh = ah + 2 * L::OP_BYTES, bl = ah + 3 * L::OP_BYTES;
+                    const uint32_t al = ah + L::OP_BYTES, bh = ah + X::kOps * L::OP_BYTES, bl = bh + L::OP_BYTES;
                     wgmma_fence();
 #pragma unroll
-                    for (int pass = 0; pass < 3; ++pass) {
+                    for (int pass = 0; pass < PASSES; ++pass) {
                         const uint32_t aa = pass == 2 ? al : ah, bb = pass == 1 ? bl : bh;
 #pragma unroll
                         for (int k4 = 0; k4 < L::KB / UMMA_K; ++k4)
-                            acc.mma_halves<1, 1>(make_desc(aa + k4 * 2048, L::KB * 128, 1024), make_desc(aa + L::KB * 128 + k4 * 2048, L::KB * 128, 1024),
-                                                 make_desc(bb + k4 * 2048, L::KB * 128, 1024), make_desc(bb + L::KB * 128 + k4 * 2048, L::KB * 128, 1024),
-                                                 (kb | pass | k4) != 0);
+                            acc.template mma_halves<1, 1, typename X::Mma>(
+                                make_desc(aa + k4 * 2048, L::KB * 128, 1024), make_desc(aa + L::KB * 128 + k4 * 2048, L::KB * 128, 1024),
+                                make_desc(bb + k4 * 2048, L::KB * 128, 1024), make_desc(bb + L::KB * 128 + k4 * 2048, L::KB * 128, 1024),
+                                (kb | pass | k4) != 0);
                     }
                     wgmma_commit();
                     wgmma_wait<1>();
@@ -666,13 +770,18 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                         const int grow = gt * a.Cout + kb * L::KB;                         // (tile, co) rows of the re-tiled grad_output
                         tma_load_2d(&tmGh, full + s, st, 0, grow);
                         tma_load_2d(&tmGh, full + s, st + L::KB * 128, 64, grow);
-                        tma_load_2d(&tmGl, full + s, st + L::OP_BYTES, 0, grow);
-                        tma_load_2d(&tmGl, full + s, st + L::OP_BYTES + L::KB * 128, 64, grow);
+                        if constexpr (X::kSplit) {
+                            tma_load_2d(&tmGl, full + s, st + L::OP_BYTES, 0, grow);
+                            tma_load_2d(&tmGl, full + s, st + L::OP_BYTES + L::KB * 128, 64, grow);
+                        }
                         const int kc0 = ((2 * h) * K + kk) * BK, kc1 = ((2 * h + 1) * K + kk) * BK;   // the chunk's two channel blocks
-                        tma_load_2d(&tmWh, full + s, st + 2 * L::OP_BYTES, kc0, kb * L::KB);
-                        tma_load_2d(&tmWh, full + s, st + 2 * L::OP_BYTES + L::KB * 128, kc1, kb * L::KB);
-                        tma_load_2d(&tmWl, full + s, st + 3 * L::OP_BYTES, kc0, kb * L::KB);
-                        tma_load_2d(&tmWl, full + s, st + 3 * L::OP_BYTES + L::KB * 128, kc1, kb * L::KB);
+                        unsigned char *sw = st + X::kOps * L::OP_BYTES;
+                        tma_load_2d(&tmWh, full + s, sw, kc0, kb * L::KB);
+                        tma_load_2d(&tmWh, full + s, sw + L::KB * 128, kc1, kb * L::KB);
+                        if constexpr (X::kSplit) {
+                            tma_load_2d(&tmWl, full + s, sw + L::OP_BYTES, kc0, kb * L::KB);
+                            tma_load_2d(&tmWl, full + s, sw + L::OP_BYTES + L::KB * 128, kc1, kb * L::KB);
+                        }
                     }
         }
     } else if (warp >= 2 && threadIdx.x < 64 + kProducerThreads) {
@@ -684,7 +793,7 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
         const int q = warp & 3, part = pwp >> 2;
         const int sub = lane >> 3, j = lane & 7;
         const uint32_t stg = smem_u32(smem + L::STG_OFF);
-        const float *xb = a.xh + (int64_t)b * a.H * a.W * a.C + j * 4;
+        const T *xb = a.xh + (int64_t)b * a.H * a.W * a.C + j * 4;
         float *gxb = a.gxh ? a.gxh + (int64_t)b * a.H * a.W * a.C + j * 4 : nullptr;
         const int R0 = q * 32;
         int rrow[2];
@@ -695,7 +804,7 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
         int n = 0, t = 0;
         for (int kk = blockIdx.y; kk < K; kk += a.tap_splits, ++t) {
             const int tb = t & 1;
-            const DcnDTab T = tab_of(tb);
+            const DcnDTab tab = tab_of(tb);
             float vh[2] = {0.f, 0.f}, vw[2] = {0.f, 0.f}, vm[2] = {0.f, 0.f};
             for (int h = 0; h < a.nch; ++h, ++n) {
                 const int buf = n & 1;
@@ -719,9 +828,9 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
 #pragma unroll
                 for (int u = 0; u < 2; ++u) {
                     const int r = rrow[u];
-                    const float4 w = T.w[r], ch = T.h[r], cv = T.v[r];
-                    const uint2 cc = T.c[r];
-                    const float mk = T.m[r];               // ch / cv carry the mask already; the scatter needs it separately
+                    const float4 w = tab.w[r], ch = tab.h[r], cv = tab.v[r];
+                    const uint2 cc = tab.c[r];
+                    const float mk = tab.m[r];               // ch / cv carry the mask already; the scatter needs it separately
                     const int y0 = (int)(cc.x & 0xffffu) * a.W, y1 = (int)(cc.x >> 16) * a.W;
                     const int x0 = (int)(cc.y & 0xffffu), x1 = (int)(cc.y >> 16);
                     const int64_t o1 = (int64_t)(y0 + x0) * a.C + h * 128, o2 = (int64_t)(y0 + x1) * a.C + h * 128;
@@ -731,10 +840,10 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                         float4 g[2], v1[2], v2[2], v3[2], v4[2];
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
-                            v1[e] = __ldg(reinterpret_cast<const float4 *>(xb + o1) + (eh + e) * 8);
-                            v2[e] = __ldg(reinterpret_cast<const float4 *>(xb + o2) + (eh + e) * 8);
-                            v3[e] = __ldg(reinterpret_cast<const float4 *>(xb + o3) + (eh + e) * 8);
-                            v4[e] = __ldg(reinterpret_cast<const float4 *>(xb + o4) + (eh + e) * 8);
+                            v1[e] = ld4_blk(xb + o1, 0, eh + e);
+                            v2[e] = ld4_blk(xb + o2, 0, eh + e);
+                            v3[e] = ld4_blk(xb + o3, 0, eh + e);
+                            v4[e] = ld4_blk(xb + o4, 0, eh + e);
                             const uint32_t ad = stg + (uint32_t)r * 512u + ((((uint32_t)(j + 8 * (eh + e))) ^ (uint32_t)(r & 31)) << 4);
                             asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(g[e].x), "=f"(g[e].y), "=f"(g[e].z), "=f"(g[e].w) : "r"(ad));
                         }
@@ -777,19 +886,33 @@ dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_
                 if (j == 0 && py < a.Ho && px < a.Wo) {
                     const int pc = py * a.Wo + px;
                     if (a.goff) {
-                        float *gp = a.goff + (int64_t)b * a.goff_bs;
-                        gp[(int64_t)(2 * kk) * a.P + pc] = vh[u];
-                        gp[(int64_t)(2 * kk + 1) * a.P + pc] = vw[u];
+                        T *gp = a.goff + (int64_t)b * a.goff_bs;
+                        gp[(int64_t)(2 * kk) * a.P + pc] = from_f32<T>(vh[u]);
+                        gp[(int64_t)(2 * kk + 1) * a.P + pc] = from_f32<T>(vw[u]);
                     }
-                    if (a.gmask) a.gmask[(int64_t)b * a.gmask_bs + (int64_t)kk * a.P + pc] = vm[u];
+                    if (a.gmask) a.gmask[(int64_t)b * a.gmask_bs + (int64_t)kk * a.P + pc] = from_f32<T>(vm[u]);
                 }
             }
         }
     }
 }
 
-// y [B][C][P] += x [B][P][C]   (the NHWC gradient scratch folded into the caller's NCHW grad_input, which is accumulated into)
-__global__ void __launch_bounds__(256) dcn_nhwc_to_nchw_add_kernel(const float *__restrict__ x, float *__restrict__ y, int C, int P) {
+__global__ void __launch_bounds__(kDcnThreads, 1)
+dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_constant__ CUtensorMap tmGl,
+                         const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, DcnDArgs a) {
+    dcn_dgrad_body<float>(tmGh, tmGl, tmWh, tmWl, a);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kDcnThreads, 1)
+dcn_dgrad_half_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmW, DcnDArgsT<T> a) {
+    dcn_dgrad_body<T>(tmG, tmG, tmW, tmW, a);
+}
+
+// y [B][C][P] += x [B][P][C]   (the NHWC gradient scratch folded into the caller's NCHW grad_input, which is accumulated into;
+// a T grad_input is rounded once, after the fp32 sum)
+template <typename T>
+__device__ __forceinline__ void nhwc_to_nchw_add_body(const float *__restrict__ x, T *__restrict__ y, int C, int P) {
     __shared__ float t[32][33];
     const int b = blockIdx.z, p0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
@@ -800,7 +923,90 @@ __global__ void __launch_bounds__(256) dcn_nhwc_to_nchw_add_kernel(const float *
     __syncthreads();
     for (int i = ty; i < 32; i += 8) {
         const int c = c0 + i, p = p0 + tx;
-        if (p < P && c < C) y[((int64_t)b * C + c) * P + p] += t[tx][i];
+        if (p < P && c < C) {
+            T &d = y[((int64_t)b * C + c) * P + p];
+            d = from_f32<T>(to_f32(d) + t[tx][i]);
+        }
+    }
+}
+__global__ void __launch_bounds__(256) dcn_nhwc_to_nchw_add_kernel(const float *__restrict__ x, float *__restrict__ y, int C, int P) {
+    nhwc_to_nchw_add_body<float>(x, y, C, P);
+}
+template <typename T>
+__global__ void __launch_bounds__(256) dcn_nhwc_to_nchw_add_half_kernel(const float *__restrict__ x, T *__restrict__ y, int C, int P) {
+    nhwc_to_nchw_add_body<T>(x, y, C, P);
+}
+
+// grad_output [B][Cout][P] T -> [B * tiles][Cout][128] T in the 8 x 16 tile order of the kernels (0 outside the map): the single
+// MMA operand of the half-precision gradient kernels
+template <typename T>
+__global__ void dcn_go_retile_half_kernel(const T *__restrict__ go, int B, int Cout, int Ho, int Wo, int tiles_x, int tiles_per_sample,
+                                          T *__restrict__ out) {
+    // one thread = one 16-pixel tile row of one channel: 32 contiguous bytes in and out
+    const int64_t n = (int64_t)B * tiles_per_sample * Cout * 8;
+    const bool vec = (Wo & 7) == 0 && ((uintptr_t)go & 15) == 0;     // 16-byte rows (a caller's view may start anywhere)
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int gr = (int)(i & 7);
+        int64_t t = i >> 3;
+        const int co = (int)(t % Cout); t /= Cout;
+        const int tile = (int)(t % tiles_per_sample);
+        const int b = (int)(t / tiles_per_sample);
+        const int py = (tile / tiles_x) * 8 + gr, px0 = (tile % tiles_x) * 16;
+        const T *src = go + ((int64_t)b * Cout + co) * Ho * Wo + (int64_t)py * Wo + px0;
+        uint4 *dst = reinterpret_cast<uint4 *>(out + i * 16);
+        if (py < Ho && vec && px0 + 16 <= Wo) {
+            dst[0] = __ldg(reinterpret_cast<const uint4 *>(src));
+            dst[1] = __ldg(reinterpret_cast<const uint4 *>(src) + 1);
+        } else {
+            uint4 v[2];
+            T *h = reinterpret_cast<T *>(v);
+#pragma unroll
+            for (int e = 0; e < 16; ++e) h[e] = (py < Ho && px0 + e < Wo) ? src[e] : from_f32<T>(0.f);
+            dst[0] = v[0]; dst[1] = v[1];
+        }
+    }
+}
+
+// weight [Cout][C][K] WT (fp32 or T) -> T [Cout][(cb * K + k) * 64 + cl]  (channel c = cb * 64 + cl), the layout of dcn_weight_pack_kernel
+template <typename WT, typename T>
+__global__ void dcn_weight_pack_half_kernel(const WT *__restrict__ w, int Cout, int C, int K, T *__restrict__ out) {
+    const int64_t n = (int64_t)Cout * C * K;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const int cl = (int)(i % 64);
+        int64_t t = i / 64;
+        const int k = (int)(t % K); t /= K;
+        const int cb = (int)(t % (C / 64));
+        const int co = (int)(t / (C / 64));
+        out[i] = from_f32<T>(to_f32(w[((int64_t)co * C + cb * 64 + cl) * K + k]));
+    }
+}
+
+template <typename WT> __global__ void dcn_to_f32_kernel(const WT *__restrict__ x, float *__restrict__ y, int64_t n) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) y[i] = to_f32(x[i]);
+}
+// y += x, rounded once to WT (the fp32 weight-gradient scratch folded into a half-precision grad_weight)
+template <typename WT> __global__ void dcn_add_f32_kernel(const float *__restrict__ x, WT *__restrict__ y, int64_t n) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        y[i] = from_f32<WT>(to_f32(y[i]) + x[i]);
+}
+
+// grad_bias[o] += sum_{b,p} grad_output[b,o,p] for T grad_output, summed in fp32 (one CTA per output channel)
+template <typename T, typename WT>
+__global__ void __launch_bounds__(256) dcn_bias_grad_half_kernel(const T *__restrict__ go, int B, int Cout, int P, WT *__restrict__ gb) {
+    const int o = blockIdx.x;
+    float acc = 0.f;
+    for (int64_t i = threadIdx.x; i < (int64_t)B * P; i += blockDim.x) {
+        const int b = (int)(i / P);
+        acc += to_f32(go[((int64_t)b * Cout + o) * P + (i - (int64_t)b * P)]);
+    }
+    __shared__ float red[32];
+    for (int s = 16; s > 0; s >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, s);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        acc = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
+        for (int s = 16; s > 0; s >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, s);
+        if (threadIdx.x == 0) gb[o] = from_f32<WT>(to_f32(gb[o]) + acc);
     }
 }
 
@@ -844,25 +1050,34 @@ __global__ void dcn_go_retile_kernel(const float *__restrict__ go, int B, int Co
     }
 }
 
-// x [B][C][P] -> y [B][P][C] (fp32), 32 x 32 tiles through shared memory; both sides 128-byte rows
-__global__ void __launch_bounds__(256)
-dcn_nchw_to_nhwc_kernel(const float *__restrict__ x, float *__restrict__ y, int C, int P) {
+// x [B][C][P] -> y [B][P][C] (fp32 or T, exact), 32 x 32 tiles through shared memory
+template <typename T>
+__device__ __forceinline__ void nchw_to_nhwc_body(const T *__restrict__ x, T *__restrict__ y, int C, int P) {
     __shared__ float tile[32][33];
     const int b = blockIdx.z, c0 = blockIdx.y * 32, p0 = blockIdx.x * 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-    const float *xb = x + (int64_t)b * C * P;
-    float *yb = y + (int64_t)b * C * P;
+    const T *xb = x + (int64_t)b * C * P;
+    T *yb = y + (int64_t)b * C * P;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         const int c = c0 + ty + 8 * j, p = p0 + tx;
-        tile[ty + 8 * j][tx] = (c < C && p < P) ? __ldg(xb + (int64_t)c * P + p) : 0.f;
+        tile[ty + 8 * j][tx] = (c < C && p < P) ? ld1(xb + (int64_t)c * P + p) : 0.f;
     }
     __syncthreads();
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         const int p = p0 + ty + 8 * j, c = c0 + tx;
-        if (p < P && c < C) yb[(int64_t)p * C + c] = tile[tx][ty + 8 * j];
+        if (p < P && c < C) yb[(int64_t)p * C + c] = from_f32<T>(tile[tx][ty + 8 * j]);
     }
+}
+__global__ void __launch_bounds__(256)
+dcn_nchw_to_nhwc_kernel(const float *__restrict__ x, float *__restrict__ y, int C, int P) {
+    nchw_to_nhwc_body<float>(x, y, C, P);
+}
+template <typename T>
+__global__ void __launch_bounds__(256)
+dcn_nchw_to_nhwc_half_kernel(const T *__restrict__ x, T *__restrict__ y, int C, int P) {
+    nchw_to_nhwc_body<T>(x, y, C, P);
 }
 
 // weight [Cout][C][K] fp32 -> hi / lo bf16 [Cout][(cb * K + k) * 64 + cl]  (channel c = cb * 64 + cl)
@@ -883,6 +1098,35 @@ __global__ void dcn_weight_pack_kernel(const float *__restrict__ w, int Cout, in
     }
 }
 
+// split-K of the fused weight gradient over the pixel tiles: whole waves of CTAs (one CTA per SM), the fewest
+// (rounds x tiles per CTA + per-CTA overhead)
+int dcn_wgrad_splits(int nkb, int Cout, int ntiles) {
+    const int ctas_fixed = nkb * (Cout / BM);
+    int splits = 1;
+    int64_t best = -1;
+    for (int waves = 1; waves <= 4; ++waves) {
+        int sp = (int)((int64_t)waves * sm_count() / ctas_fixed);
+        sp = sp < 1 ? 1 : (sp > ntiles ? ntiles : sp);
+        const int64_t rounds = ceil_div((int64_t)ctas_fixed * sp, sm_count());
+        const int64_t cost = rounds * (ceil_div(ntiles, sp) + 3);
+        if (best < 0 || cost < best) { best = cost; splits = sp; }
+    }
+    return splits;
+}
+
+// taps of the fused data gradient spread over grid.y (a divisor of the tap count): the fewest (rounds of CTAs x N blocks per
+// CTA + per-CTA overhead)
+int dcn_dgrad_tap_splits(int K, int ntiles, int nch) {
+    int splits = 1;
+    int64_t best = -1;
+    for (int sp = 1; sp <= K; ++sp) {
+        if (K % sp) continue;
+        const int64_t cost = ceil_div((int64_t)ntiles * sp, sm_count()) * ((int64_t)(K / sp) * nch + 1);
+        if (best < 0 || cost < best) { best = cost; splits = sp; }
+    }
+    return splits;
+}
+
 // launch of the fused weight gradient once the NHWC input and the re-tiled grad_output exist
 int launch_dcn_wgrad(DcnWArgs &a, const bf16 *ghi, const bf16 *glo, cudaStream_t st) {
     CUtensorMap th, tl;
@@ -890,17 +1134,7 @@ int launch_dcn_wgrad(DcnWArgs &a, const bf16 *ghi, const bf16 *glo, cudaStream_t
     if (rc) return rc;
     rc = make_map(&tl, glo, BM, (int64_t)a.ntiles * a.Cout, BM, BK, BM);
     if (rc) return rc;
-    // split-K over the pixel tiles: whole waves of CTAs (one CTA per SM), the fewest (rounds x tiles per CTA + per-CTA overhead)
-    const int ctas_fixed = a.nkb * (a.Cout / BM);
-    int splits = 1;
-    int64_t best = -1;
-    for (int waves = 1; waves <= 4; ++waves) {
-        int sp = (int)((int64_t)waves * sm_count() / ctas_fixed);
-        sp = sp < 1 ? 1 : (sp > a.ntiles ? a.ntiles : sp);
-        const int64_t rounds = ceil_div((int64_t)ctas_fixed * sp, sm_count());
-        const int64_t cost = rounds * (ceil_div(a.ntiles, sp) + 3);
-        if (best < 0 || cost < best) { best = cost; splits = sp; }
-    }
+    const int splits = dcn_wgrad_splits(a.nkb, a.Cout, a.ntiles);
     a.splits = splits;
     { int rc_attr = ensure_dyn_smem((const void *)dcn_wgrad_tcgen05_kernel, DcnWSmem::TOTAL, "dcn_wgrad_tcgen05 smem attr"); if (rc_attr) return rc_attr; }
     dim3 grid((unsigned)a.nkb, (unsigned)splits, (unsigned)(a.Cout / BM));
@@ -918,6 +1152,173 @@ int launch_dcn_fwd(const CUtensorMap &th, const CUtensorMap &tl, const DcnFArgs 
     dim3 grid((unsigned)(a.B * a.tiles_per_sample), (unsigned)(a.Cout / BN), 1);
     kern<<<grid, kDcnThreads, smem, st>>>(th, tl, a);
     return check_launch("dcn_fwd_tcgen05_kernel");
+}
+
+// ---------------------------------------------------------------- half precision (T = __half / bf16, weights WT = float or T)
+// Workspace pieces, each 256-byte aligned.  Forward: NHWC T input, packed T weights, fp32 bias.  Backward: NHWC T input, fp32 NHWC
+// grad_input scratch, re-tiled T grad_output, packed T weights, fp32 grad_weight scratch (used when WT = T).
+struct DcnHalfWs {
+    int64_t x, gx, g, w, gw, bias;
+    DcnHalfWs(int64_t B, int64_t C, int64_t H, int64_t W, int64_t Cout, int64_t Ho, int64_t Wo, int64_t kh, int64_t kw) {
+        const int64_t tiles = ceil_div(Wo, 16) * ceil_div(Ho, 8);
+        x = round_up(B * H * W * C * 2, 256);
+        gx = round_up(B * H * W * C * 4, 256);
+        g = round_up(B * tiles * Cout * BM * 2, 256);
+        w = round_up(Cout * C * kh * kw * 2, 256);
+        gw = round_up(Cout * C * kh * kw * 4, 256);
+        bias = round_up(Cout * 4, 256);
+    }
+    int64_t forward() const { return x + w + bias; }
+    int64_t backward() const { return x + gx + g + w + gw; }
+};
+
+inline unsigned grid_cap(int64_t n, int per_sm) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), (int64_t)sm_count() * per_sm)); }
+
+template <typename T>
+int dcn_to_nhwc_half(const T *input, T *xh, int B, int C, int H, int W, cudaStream_t st) {
+    dim3 tg((unsigned)ceil_div((int64_t)H * W, 32), (unsigned)ceil_div(C, 32), (unsigned)B);
+    dcn_nchw_to_nhwc_half_kernel<T><<<tg, 256, 0, st>>>(input, xh, C, H * W);
+    return check_launch("dcn_nchw_to_nhwc_half_kernel");
+}
+
+template <typename T, typename WT>
+int dcn_pack_weight_half(const WT *weight, T *wp, int Cout, int C, int K, cudaStream_t st) {
+    const int64_t nw = (int64_t)Cout * C * K;
+    dcn_weight_pack_half_kernel<WT, T><<<grid_cap(nw, 8), 256, 0, st>>>(weight, Cout, C, K, wp);
+    return check_launch("dcn_weight_pack_half_kernel");
+}
+
+template <typename T, typename WT>
+int dcn_forward_half(const T *input, const WT *weight, const WT *bias, const T *offset, int64_t offset_bstride, const T *mask,
+                     int64_t mask_bstride, T *output, unsigned char *ws, int B, int C, int H, int W, int Cout, int kh, int kw, int sh,
+                     int sw, int ph, int pw, int dh, int dw, cudaStream_t st) {
+    DcnFArgsT<T> a;
+    a.B = B; a.C = C; a.H = H; a.W = W; a.Cout = Cout; a.kh = kh; a.kw = kw; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw;
+    a.dh = dh; a.dw = dw;
+    a.Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1;
+    a.Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
+    a.P = a.Ho * a.Wo;
+    a.tiles_x = (int)ceil_div(a.Wo, 16);
+    a.tiles_per_sample = a.tiles_x * (int)ceil_div(a.Ho, 8);
+    a.ncb = C / BK; a.nkb = kh * kw * a.ncb;
+    const DcnHalfWs L(B, C, H, W, Cout, a.Ho, a.Wo, kh, kw);
+    T *xh = (T *)ws, *wp = (T *)(ws + L.x);
+    float *bf = (float *)(ws + L.x + L.w);
+    int rc = dcn_to_nhwc_half(input, xh, B, C, H, W, st);
+    if (rc) return rc;
+    if ((rc = dcn_pack_weight_half(weight, wp, Cout, C, kh * kw, st))) return rc;
+    const float *b32 = nullptr;
+    if constexpr (std::is_same<WT, float>::value) {
+        b32 = bias;
+        (void)bf;
+    } else if (bias) {
+        dcn_to_f32_kernel<WT><<<1, 256, 0, st>>>(bias, bf, Cout);
+        if ((rc = check_launch("dcn_to_f32_kernel"))) return rc;
+        b32 = bf;
+    }
+    a.xh = xh; a.off = offset; a.msk = mask; a.bias = b32; a.out = output; a.off_bs = offset_bstride; a.mask_bs = mask_bstride;
+    CUtensorMap tw;
+    const int64_t Kt = (int64_t)kh * kw * C;
+    if ((rc = make_map(&tw, wp, Kt, Cout, Kt, BK, 128))) return rc;      // 2-byte elements: the bf16 map type only sets the size
+    const int smem = DcnSmem<128, 2, 1>::total(kh * kw);
+    if (smem > 227 * 1024) return MR_ERR_UNSUPPORTED;
+    { int rc_attr = ensure_dyn_smem((const void *)dcn_fwd_half_kernel<T>, smem, "dcn_fwd_half smem attr"); if (rc_attr) return rc_attr; }
+    dim3 grid((unsigned)(a.B * a.tiles_per_sample), (unsigned)(a.Cout / 128), 1);
+    dcn_fwd_half_kernel<T><<<grid, kDcnThreads, smem, st>>>(tw, a);
+    return check_launch("dcn_fwd_half_kernel");
+}
+
+template <typename T, typename WT>
+int dcn_backward_half(const T *input, const WT *weight, const T *offset, int64_t offset_bstride, const T *mask, int64_t mask_bstride,
+                      const T *grad_output, T *grad_input, WT *grad_weight, WT *grad_bias, T *grad_offset, int64_t grad_offset_bstride,
+                      T *grad_mask, int64_t grad_mask_bstride, float scale, unsigned char *ws, int B, int C, int H, int W, int Cout,
+                      int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, cudaStream_t st) {
+    const int Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1, Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
+    const int tiles_x = (int)ceil_div(Wo, 16), tiles_per_sample = tiles_x * (int)ceil_div(Ho, 8), ntiles = B * tiles_per_sample;
+    const int K = kh * kw;
+    const DcnHalfWs L(B, C, H, W, Cout, Ho, Wo, kh, kw);
+    T *xh = (T *)ws;
+    float *gxh = (float *)(ws + L.x);
+    T *gt = (T *)(ws + L.x + L.gx);
+    T *wp = (T *)(ws + L.x + L.gx + L.g);
+    float *gw32 = (float *)(ws + L.x + L.gx + L.g + L.w);
+    const bool want_data = grad_input || grad_offset || grad_mask;
+    int rc = MR_OK;
+    if (grad_bias) {
+        dcn_bias_grad_half_kernel<T, WT><<<Cout, 256, 0, st>>>(grad_output, B, Cout, Ho * Wo, grad_bias);
+        if ((rc = check_launch("dcn_bias_grad_half_kernel"))) return rc;
+    }
+    if (!want_data && !grad_weight) return MR_OK;
+    if ((rc = dcn_to_nhwc_half(input, xh, B, C, H, W, st))) return rc;
+    const int64_t ng = (int64_t)ntiles * Cout * 8;
+    dcn_go_retile_half_kernel<T><<<grid_cap(ng, 16), 256, 0, st>>>(grad_output, B, Cout, Ho, Wo, tiles_x, tiles_per_sample, gt);
+    if ((rc = check_launch("dcn_go_retile_half_kernel"))) return rc;
+    if (grad_weight) {
+        constexpr bool f32w = std::is_same<WT, float>::value;
+        const int64_t nw = (int64_t)Cout * C * K;
+        if constexpr (!f32w) MR_CUDA_TRY(cudaMemsetAsync(gw32, 0, (size_t)nw * 4, st), "cudaMemsetAsync(dcn grad_weight scratch)");
+        DcnWArgsT<T> a;
+        a.B = B; a.C = C; a.H = H; a.W = W; a.Cout = Cout; a.kh = kh; a.kw = kw; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw; a.dh = dh; a.dw = dw;
+        a.Ho = Ho; a.Wo = Wo; a.P = Ho * Wo; a.tiles_x = tiles_x; a.tiles_per_sample = tiles_per_sample; a.ncb = C / BK; a.nkb = K * a.ncb;
+        a.ntiles = ntiles;
+        a.xh = xh; a.off = offset; a.msk = mask; a.off_bs = offset_bstride; a.mask_bs = mask_bstride; a.scale = scale;
+        a.gw = f32w ? (float *)grad_weight : gw32;
+        CUtensorMap tg;
+        if ((rc = make_map(&tg, gt, BM, (int64_t)ntiles * Cout, BM, BK, BM))) return rc;
+        a.splits = dcn_wgrad_splits(a.nkb, Cout, ntiles);
+        constexpr int smem = DcnWSmemT<1>::TOTAL;
+        { int rc_attr = ensure_dyn_smem((const void *)dcn_wgrad_half_kernel<T>, smem, "dcn_wgrad_half smem attr"); if (rc_attr) return rc_attr; }
+        dim3 grid((unsigned)a.nkb, (unsigned)a.splits, (unsigned)(Cout / BM));
+        dcn_wgrad_half_kernel<T><<<grid, kDcnThreads, smem, st>>>(tg, a);
+        if ((rc = check_launch("dcn_wgrad_half_kernel"))) return rc;
+        if constexpr (!f32w) {
+            dcn_add_f32_kernel<WT><<<grid_cap(nw, 8), 256, 0, st>>>(gw32, grad_weight, nw);
+            if ((rc = check_launch("dcn_add_f32_kernel"))) return rc;
+        }
+    }
+    if (want_data) {
+        if ((rc = dcn_pack_weight_half(weight, wp, Cout, C, K, st))) return rc;
+        if (grad_input) MR_CUDA_TRY(cudaMemsetAsync(gxh, 0, (size_t)B * H * W * C * 4, st), "cudaMemsetAsync(dcn grad_input scratch)");
+        DcnDArgsT<T> a;
+        a.B = B; a.C = C; a.H = H; a.W = W; a.Cout = Cout; a.kh = kh; a.kw = kw; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw; a.dh = dh; a.dw = dw;
+        a.Ho = Ho; a.Wo = Wo; a.P = Ho * Wo; a.tiles_x = tiles_x; a.tiles_per_sample = tiles_per_sample; a.nch = C / 128;
+        a.nkk = Cout / DcnDSmemT<1>::KB;
+        a.xh = xh; a.off = offset; a.msk = mask; a.gxh = grad_input ? gxh : nullptr; a.goff = grad_offset; a.gmask = grad_mask;
+        a.off_bs = offset_bstride; a.mask_bs = mask_bstride; a.goff_bs = grad_offset_bstride; a.gmask_bs = grad_mask_bstride;
+        a.tap_splits = dcn_dgrad_tap_splits(K, ntiles, a.nch);
+        CUtensorMap tg, tw;
+        if ((rc = make_map(&tg, gt, BM, (int64_t)ntiles * Cout, BM, BK, DcnDSmemT<1>::KB))) return rc;
+        if ((rc = make_map(&tw, wp, (int64_t)K * C, Cout, (int64_t)K * C, BK, DcnDSmemT<1>::KB))) return rc;
+        constexpr int smem = DcnDSmemT<1>::TOTAL;
+        { int rc_attr = ensure_dyn_smem((const void *)dcn_dgrad_half_kernel<T>, smem, "dcn_dgrad_half smem attr"); if (rc_attr) return rc_attr; }
+        dim3 grid((unsigned)ntiles, (unsigned)a.tap_splits);
+        dcn_dgrad_half_kernel<T><<<grid, kDcnThreads, smem, st>>>(tg, tw, a);
+        if ((rc = check_launch("dcn_dgrad_half_kernel"))) return rc;
+        if (grad_input) {
+            dim3 tgr((unsigned)ceil_div((int64_t)H * W, 32), (unsigned)ceil_div(C, 32), (unsigned)B);
+            dcn_nhwc_to_nchw_add_half_kernel<T><<<tgr, 256, 0, st>>>(gxh, grad_input, C, H * W);
+            if ((rc = check_launch("dcn_nhwc_to_nchw_add_half_kernel"))) return rc;
+        }
+    }
+    return MR_OK;
+}
+
+// dtype codes of the C-ABI: 0 = fp32, 1 = bf16, 2 = fp16
+enum { kDtF32 = 0, kDtBF16 = 1, kDtF16 = 2 };
+
+// the fused-path conditions shared by the half-precision entry points; MR_OK when the call may go ahead
+int dcn_half_eligible(int dtype, int weight_dtype, int B, int C, int H, int W, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
+                      int dh, int dw, int group, int dg) {
+    if (dtype != kDtBF16 && dtype != kDtF16) return MR_ERR_UNSUPPORTED;
+    if (weight_dtype != kDtF32 && weight_dtype != dtype) return MR_ERR_UNSUPPORTED;
+    if (group != 1 || dg != 1 || C % 64 || Cout % 128 || B <= 0 || H > 65535 || W > 65535) return MR_ERR_UNSUPPORTED;
+    if (getenv("MR_DCN_UNFUSED")) return MR_ERR_UNSUPPORTED;
+    if (kh <= 0 || kw <= 0 || sh <= 0 || sw <= 0 || dh <= 0 || dw <= 0 || ph < 0 || pw < 0 || C <= 0 || H <= 0 || W <= 0) return MR_ERR_BAD_SHAPE;
+    const int Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1, Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
+    if (Ho <= 0 || Wo <= 0) return MR_ERR_BAD_SHAPE;
+    const int64_t ntiles = (int64_t)B * ceil_div(Wo, 16) * ceil_div(Ho, 8);
+    if (ntiles * Cout > 0x7fffffffLL) return MR_ERR_UNSUPPORTED;
+    return MR_OK;
 }
 
 }  // namespace
@@ -1042,14 +1443,7 @@ int mr_dcn_backward_fused_f32(const float *input, const float *weight, const flo
         a.xh = xh; a.off = offset; a.msk = mask; a.gxh = grad_input ? gxh : nullptr; a.goff = grad_offset; a.gmask = grad_mask;
         a.off_bs = offset_bstride; a.mask_bs = mask_bstride; a.goff_bs = grad_offset_bstride; a.gmask_bs = grad_mask_bstride;
         const int K = kh * kw;
-        // taps are spread over grid.y (a divisor of the tap count): the fewest (rounds of CTAs x N blocks per CTA + per-CTA overhead)
-        int splits = 1;
-        int64_t best = -1;
-        for (int sp = 1; sp <= K; ++sp) {
-            if (K % sp) continue;
-            const int64_t cost = ceil_div((int64_t)ntiles * sp, sm_count()) * ((int64_t)(K / sp) * a.nch + 1);
-            if (best < 0 || cost < best) { best = cost; splits = sp; }
-        }
+        const int splits = dcn_dgrad_tap_splits(K, ntiles, a.nch);
         a.tap_splits = splits;
         CUtensorMap gh, gl, wh, wl;
         const int64_t Kt = (int64_t)K * C;
@@ -1118,5 +1512,60 @@ int mr_dcn_wgrad_fused_f32(const float *input, const float *offset, int64_t offs
     a.xh = xh; a.off = offset; a.msk = mask; a.off_bs = offset_bstride; a.mask_bs = mask_bstride; a.gw = grad_weight; a.scale = scale;
     return launch_dcn_wgrad(a, ghi, glo, st);
 }
+
+/* ---- half precision: dtype 1 = bf16, 2 = fp16 for input / offset / mask / output / grad_output / grad_input / grad_offset /
+ * grad_mask; weight_dtype 0 = fp32 or the same code as dtype for weight / bias / grad_weight / grad_bias. */
+int64_t mr_dcn_fused_workspace_bytes_h(int64_t B, int64_t C, int64_t H, int64_t W, int64_t Cout, int64_t kh, int64_t kw) {
+    return DcnHalfWs(B, C, H, W, Cout, 1, 1, kh, kw).forward();
+}
+
+int64_t mr_dcn_fused_backward_workspace_bytes_h(int64_t B, int64_t C, int64_t H, int64_t W, int64_t Cout, int64_t Ho, int64_t Wo,
+                                                int64_t kh, int64_t kw) {
+    return DcnHalfWs(B, C, H, W, Cout, Ho, Wo, kh, kw).backward();
+}
+
+#define MR_DCN_HALF_DISPATCH(CALL)                                                                                       \
+    if (dtype == kDtBF16 && weight_dtype == kDtF32) { typedef bf16 T; typedef float WT; return CALL; }                   \
+    if (dtype == kDtBF16) { typedef bf16 T; typedef bf16 WT; return CALL; }                                              \
+    if (weight_dtype == kDtF32) { typedef __half T; typedef float WT; return CALL; }                                     \
+    { typedef __half T; typedef __half WT; return CALL; }
+
+int mr_dcn_forward_fused_h(const void *input, const void *weight, const void *bias, const void *offset, int64_t offset_bstride,
+                           const void *mask, int64_t mask_bstride, void *output, void *workspace, int64_t workspace_bytes, int B,
+                           int C, int H, int W, int Cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int group,
+                           int dg, int dtype, int weight_dtype, void *stream) {
+    int rc = dcn_half_eligible(dtype, weight_dtype, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg);
+    if (rc) return rc;
+    if (!input || !weight || !offset || !output || !workspace) return MR_ERR_NULL_POINTER;
+    if (workspace_bytes < mr_dcn_fused_workspace_bytes_h(B, C, H, W, Cout, kh, kw) || ((uintptr_t)workspace % 256)) return MR_ERR_UNSUPPORTED;
+    MR_DCN_HALF_DISPATCH((dcn_forward_half<T, WT>((const T *)input, (const WT *)weight, (const WT *)bias, (const T *)offset, offset_bstride,
+                                                  (const T *)mask, mask_bstride, (T *)output, (unsigned char *)workspace, B, C, H, W, Cout,
+                                                  kh, kw, sh, sw, ph, pw, dh, dw, (cudaStream_t)stream)))
+}
+
+/* grad_input / grad_weight / grad_bias accumulate, grad_offset / grad_mask are assigned, as in mr_dcn_backward_f32.  The data
+ * gradients need C % 128 == 0: a call that wants one of them with C % 128 != 0 returns MR_ERR_UNSUPPORTED before any work. */
+int mr_dcn_backward_fused_h(const void *input, const void *weight, const void *offset, int64_t offset_bstride, const void *mask,
+                            int64_t mask_bstride, const void *grad_output, void *grad_input, void *grad_weight, void *grad_bias,
+                            void *grad_offset, int64_t grad_offset_bstride, void *grad_mask, int64_t grad_mask_bstride,
+                            float weight_grad_scale, void *workspace, int64_t workspace_bytes, int B, int C, int H, int W, int Cout,
+                            int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int group, int dg, int dtype,
+                            int weight_dtype, void *stream) {
+    int rc = dcn_half_eligible(dtype, weight_dtype, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg);
+    if (rc) return rc;
+    const bool want_data = grad_input || grad_offset || grad_mask;
+    if (want_data && (C % 128 || getenv("MR_DCN_UNFUSED_DGRAD"))) return MR_ERR_UNSUPPORTED;
+    if (grad_weight && getenv("MR_DCN_UNFUSED_WGRAD")) return MR_ERR_UNSUPPORTED;
+    if (!input || !weight || !offset || !grad_output || !workspace) return MR_ERR_NULL_POINTER;
+    const int Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1, Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
+    if (workspace_bytes < mr_dcn_fused_backward_workspace_bytes_h(B, C, H, W, Cout, Ho, Wo, kh, kw) || ((uintptr_t)workspace % 256))
+        return MR_ERR_UNSUPPORTED;
+    MR_DCN_HALF_DISPATCH((dcn_backward_half<T, WT>((const T *)input, (const WT *)weight, (const T *)offset, offset_bstride, (const T *)mask,
+                                                   mask_bstride, (const T *)grad_output, (T *)grad_input, (WT *)grad_weight, (WT *)grad_bias,
+                                                   (T *)grad_offset, grad_offset_bstride, (T *)grad_mask, grad_mask_bstride,
+                                                   weight_grad_scale, (unsigned char *)workspace, B, C, H, W, Cout, kh, kw, sh, sw, ph,
+                                                   pw, dh, dw, (cudaStream_t)stream)))
+}
+#undef MR_DCN_HALF_DISPATCH
 
 }  // extern "C"

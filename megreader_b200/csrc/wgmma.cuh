@@ -6,6 +6,8 @@
 #include "common.cuh"
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <type_traits>
 
 namespace {
 using namespace mr;
@@ -56,67 +58,83 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int PENDING> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
 
-// D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 operands through shared-memory descriptors, fp32 accumulator fragment in
-// registers.  TA / TB = 1: the operand is MN-major in shared memory (the instruction's transpose bits).
-template <int N> struct Wgmma;
-template <> struct Wgmma<32> {
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], 16-bit operands of element type E (bf16, the default, or __half) through
+// shared-memory descriptors, fp32 accumulator fragment in registers.  TA / TB = 1: the operand is MN-major in shared memory
+// (the instruction's transpose bits).
+template <typename E> struct WgmmaElem;
+template <> struct WgmmaElem<bf16> { static constexpr bool f16 = false; };
+template <> struct WgmmaElem<__half> { static constexpr bool f16 = true; };
+template <int N, typename E = bf16> struct Wgmma;
+template <typename E> struct Wgmma<32, E> {
     template <int TA, int TB>
     static __device__ __forceinline__ void mma(float (&d)[16], uint64_t ad, uint64_t bd, uint32_t scale_d) {
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "setp.ne.b32 p, %18, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-            "%16, %17, p, 1, 1, %19, %20;\n"
-            "}\n"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-            : "l"(ad), "l"(bd), "r"(scale_d), "n"(TA), "n"(TB));
+#define MR_WGMMA_M64N32K16(AB) \
+        asm volatile( \
+            "{\n" \
+            ".reg .pred p;\n" \
+            "setp.ne.b32 p, %18, 0;\n" \
+            "wgmma.mma_async.sync.aligned.m64n32k16.f32." AB "." AB " " \
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, " \
+            "%16, %17, p, 1, 1, %19, %20;\n" \
+            "}\n" \
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]) \
+            : "l"(ad), "l"(bd), "r"(scale_d), "n"(TA), "n"(TB))
+        if constexpr (WgmmaElem<E>::f16) MR_WGMMA_M64N32K16("f16");
+        else MR_WGMMA_M64N32K16("bf16");
+#undef MR_WGMMA_M64N32K16
     }
 };
-template <> struct Wgmma<64> {
+template <typename E> struct Wgmma<64, E> {
     template <int TA, int TB>
     static __device__ __forceinline__ void mma(float (&d)[32], uint64_t ad, uint64_t bd, uint32_t scale_d) {
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "setp.ne.b32 p, %34, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-            "%32, %33, p, 1, 1, %35, %36;\n"
-            "}\n"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-            : "l"(ad), "l"(bd), "r"(scale_d), "n"(TA), "n"(TB));
+#define MR_WGMMA_M64N64K16(AB) \
+        asm volatile( \
+            "{\n" \
+            ".reg .pred p;\n" \
+            "setp.ne.b32 p, %34, 0;\n" \
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32." AB "." AB " " \
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, " \
+            "%32, %33, p, 1, 1, %35, %36;\n" \
+            "}\n" \
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]) \
+            : "l"(ad), "l"(bd), "r"(scale_d), "n"(TA), "n"(TB))
+        if constexpr (WgmmaElem<E>::f16) MR_WGMMA_M64N64K16("f16");
+        else MR_WGMMA_M64N64K16("bf16");
+#undef MR_WGMMA_M64N64K16
     }
 };
-template <> struct Wgmma<128> {
+template <typename E> struct Wgmma<128, E> {
     template <int TA, int TB>
     static __device__ __forceinline__ void mma(float (&d)[64], uint64_t ad, uint64_t bd, uint32_t scale_d) {
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "setp.ne.b32 p, %66, 0;\n"
-            "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-            "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
-            "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-            "%64, %65, p, 1, 1, %67, %68;\n"
-            "}\n"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-            : "l"(ad), "l"(bd), "r"(scale_d), "n"(TA), "n"(TB));
+#define MR_WGMMA_M64N128K16(AB) \
+        asm volatile( \
+            "{\n" \
+            ".reg .pred p;\n" \
+            "setp.ne.b32 p, %66, 0;\n" \
+            "wgmma.mma_async.sync.aligned.m64n128k16.f32." AB "." AB " " \
+            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, " \
+            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, " \
+            "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, " \
+            "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, " \
+            "%64, %65, p, 1, 1, %67, %68;\n" \
+            "}\n" \
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), \
+              "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), \
+              "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), \
+              "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), \
+              "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), \
+              "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), \
+              "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), \
+              "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]) \
+            : "l"(ad), "l"(bd), "r"(scale_d), "n"(TA), "n"(TB))
+        if constexpr (WgmmaElem<E>::f16) MR_WGMMA_M64N128K16("f16");
+        else MR_WGMMA_M64N128K16("bf16");
+#undef MR_WGMMA_M64N128K16
     }
 };
 
@@ -128,20 +146,20 @@ template <int BN> struct AccTile {
     static constexpr int LD = BN + 1;
     static constexpr int BYTES = BM * LD * 4;
     float d[2][BN / 2];
-    template <int TA, int TB>
+    template <int TA, int TB, typename E = bf16>
     __device__ __forceinline__ void mma(uint64_t a_lo, uint64_t a_hi, uint64_t b, uint32_t accumulate) {
-        Wgmma<BN>::template mma<TA, TB>(d[0], a_lo, b, accumulate);
-        Wgmma<BN>::template mma<TA, TB>(d[1], a_hi, b, accumulate);
+        Wgmma<BN, E>::template mma<TA, TB>(d[0], a_lo, b, accumulate);
+        Wgmma<BN, E>::template mma<TA, TB>(d[1], a_hi, b, accumulate);
     }
     // The same step as four 64-column instructions (b_lo / b_hi: the operand's two 64-column halves), for kernels whose
     // 768 threads leave too few registers per thread for the operands of one 128-column instruction.
-    template <int TA, int TB>
+    template <int TA, int TB, typename E = bf16>
     __device__ __forceinline__ void mma_halves(uint64_t a_lo, uint64_t a_hi, uint64_t b_lo, uint64_t b_hi, uint32_t accumulate) {
         static_assert(BN == 128, "two 64-column halves");
 #pragma unroll
         for (int half = 0; half < 2; ++half) {
-            Wgmma<64>::template mma<TA, TB>(reinterpret_cast<float (&)[32]>(d[half][0]), half ? a_hi : a_lo, b_lo, accumulate);
-            Wgmma<64>::template mma<TA, TB>(reinterpret_cast<float (&)[32]>(d[half][32]), half ? a_hi : a_lo, b_hi, accumulate);
+            Wgmma<64, E>::template mma<TA, TB>(reinterpret_cast<float (&)[32]>(d[half][0]), half ? a_hi : a_lo, b_lo, accumulate);
+            Wgmma<64, E>::template mma<TA, TB>(reinterpret_cast<float (&)[32]>(d[half][32]), half ? a_hi : a_lo, b_hi, accumulate);
         }
     }
     // fragment layout of wgmma m64nNk16: warp w of the warpgroup holds rows 16w..16w+15; d[4j + 2h + e] is row

@@ -2,6 +2,17 @@
 reference's pybind module `assets.ops.dcn.deform_conv_cuda` (assets/ops/dcn/src/deform_conv_cuda.cpp:681-695), the
 autograd Functions (assets/ops/dcn/functions/deform_conv.py:8-181) and the nn.Modules
 (assets/ops/dcn/modules/deform_conv.py:10-157).  Arithmetic: megreader_b200/csrc/dcn.cu through the C-ABI.
+
+Dtypes: the dtype of the input `x` is the compute dtype.
+  x float32                  weight / bias float32           -> the fp32 kernels, output and gradients float32
+  x float16 or bfloat16 (T)  weight / bias T or float32      -> the half-precision fused kernels (csrc/dcn_tcgen05.cu): output,
+                                                                grad_input / grad_offset / grad_mask in T, grad_weight /
+                                                                grad_bias in the weight's dtype (fp32 accumulation throughout)
+  anything else                                              -> RuntimeError naming the dtypes
+offset and mask are converted to x's dtype first (under torch.autocast the offset conv returns half precision even for an fp32
+x; upcasting is lossless).  Half-precision shapes outside the fused path (groups, deformable groups > 1, C % 64 != 0; C % 128
+!= 0 for the data gradient) are rare -- none of the reference's trunks has one -- and run the fp32 kernels on fp32 copies, with
+the results converted back.
 """
 import math
 
@@ -46,19 +57,53 @@ def _workspace(x, C, kh, kw, Ho, Wo, Cout=0, backward=False):
     return torch.empty(nbytes // 4, dtype=torch.float32, device=x.device), nbytes
 
 
-def _check(x, weight):
+_HALF_CODE = {torch.bfloat16: 1, torch.float16: 2}   # dtype codes of the C-ABI (0 = float32)
+
+
+def _check(x, weight, bias=None):
     if not x.is_cuda:
         raise RuntimeError("Not implemented on the CPU")
-    if x.dtype != torch.float32:
-        raise RuntimeError("megreader_b200 dcn: float32 only, got %s" % x.dtype)
+    wd = weight.dtype
+    ok = wd == torch.float32 if x.dtype == torch.float32 else x.dtype in _HALF_CODE and wd in (x.dtype, torch.float32)
+    if not ok or (bias is not None and bias.dtype != wd):
+        raise RuntimeError("megreader_b200 dcn: unsupported dtypes: input %s, weight %s%s (a float32 input needs float32 "
+                           "weight and bias; a float16 / bfloat16 input needs weight and bias both in its dtype or both "
+                           "float32)" % (x.dtype, wd, "" if bias is None else ", bias %s" % bias.dtype))
     if not x.is_contiguous():
         raise RuntimeError("input tensor has to be contiguous")          # deform_conv_cuda.cpp:493
     if not weight.is_contiguous():
         raise RuntimeError("weight tensor has to be contiguous")         # deform_conv_cuda.cpp:494
 
 
+def _codes(x, weight):
+    """(dtype, weight_dtype) codes of the half-precision C entry points."""
+    return _HALF_CODE[x.dtype], 0 if weight.dtype == torch.float32 else _HALF_CODE[weight.dtype]
+
+
+def _half_workspace(x, nbytes):
+    return torch.empty(int(nbytes), dtype=torch.uint8, device=x.device)
+
+
+def _in_dtype(t, dtype):
+    """t itself when it has `dtype` (or is None), else a copy in `dtype` that _write_back returns to t."""
+    return t if t is None or t.dtype == dtype else t.to(dtype)
+
+
+def _write_back(pairs):
+    for t, tc in pairs:
+        if tc is not t:
+            t.copy_(tc)
+
+
+def _float(t):
+    return None if t is None else t.float()
+
+
 def _forward(x, weight, bias, offset, mask, output, kh, kw, sh, sw, ph, pw, dh, dw, group, dg):
-    _check(x, weight)
+    _check(x, weight, bias)
+    offset, mask = offset.to(x.dtype), _in_dtype(mask, x.dtype)
+    if output.dtype != x.dtype:
+        raise RuntimeError("megreader_b200 dcn: output is %s, input %s" % (output.dtype, x.dtype))
     B, C, H, W = x.shape
     Cout = weight.size(0)
     if weight.size(2) != kh or weight.size(3) != kw:
@@ -67,11 +112,30 @@ def _forward(x, weight, bias, offset, mask, output, kh, kw, sh, sw, ph, pw, dh, 
     if C != weight.size(1) * group:
         raise RuntimeError("Input shape and kernel channels wont match: (%d vs %d)." % (C, weight.size(1) * group))
     Ho, Wo = _out_hw(H, W, kh, kw, sh, sw, ph, pw, dh, dw)
+    offset_in, mask_in = offset, mask
     offset, obs = _slab(offset)
     mbs = 0
     if mask is not None:
         mask, mbs = _slab(mask)
     assert output.is_contiguous() and output.numel() == B * Cout * Ho * Wo
+    if x.dtype != torch.float32:
+        code, wcode = _codes(x, weight)
+        ws_bytes = _lib.lib().mr_dcn_fused_workspace_bytes_h(B, C, H, W, Cout, kh, kw)
+        ws = _half_workspace(x, ws_bytes)
+        p = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        with torch.cuda.device(x.device):
+            rc = _lib.lib().mr_dcn_forward_fused_h(
+                x.data_ptr(), weight.data_ptr(), p(bias), offset.data_ptr(), obs, p(mask), mbs, output.data_ptr(),
+                ws.data_ptr(), ws_bytes, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg, code, wcode, _stream())
+        if rc != _lib.MR_ERR_UNSUPPORTED:
+            _lib.check(rc, "dcn_forward")
+            return
+        # outside the fused path: the fp32 kernels on fp32 copies
+        out32 = torch.empty(output.shape, dtype=torch.float32, device=output.device)
+        _forward(x.float(), weight.float(), _float(bias), offset_in.float(), _float(mask_in), out32, kh, kw, sh, sw, ph, pw,
+                 dh, dw, group, dg)
+        output.copy_(out32)
+        return
     ws, ws_bytes = _workspace(x, C, kh, kw, Ho, Wo, Cout)
     with torch.cuda.device(x.device):
         _lib.check(_lib.lib().mr_dcn_forward_f32(
@@ -83,9 +147,25 @@ def _forward(x, weight, bias, offset, mask, output, kh, kw, sh, sw, ph, pw, dh, 
 def _backward(x, weight, offset, mask, grad_output, grad_input, grad_weight, grad_bias, grad_offset, grad_mask,
               scale, kh, kw, sh, sw, ph, pw, dh, dw, group, dg):
     _check(x, weight)
+    if grad_input is not None and grad_input.dtype != x.dtype:
+        raise RuntimeError("megreader_b200 dcn: grad_input is %s, input %s" % (grad_input.dtype, x.dtype))
+    for g in (grad_weight, grad_bias):
+        if g is not None and g.dtype != weight.dtype:
+            raise RuntimeError("megreader_b200 dcn: weight gradients are %s, weight %s" % (g.dtype, weight.dtype))
+    # offset / mask (and their gradients) in x's dtype; gradients allocated in another dtype get the result copied back
+    offset, mask, grad_output = offset.to(x.dtype), _in_dtype(mask, x.dtype), grad_output.to(x.dtype)
+    goff_c, gmask_c = _in_dtype(grad_offset, x.dtype), _in_dtype(grad_mask, x.dtype)
+    _backward_same_dtype(x, weight, offset, mask, grad_output, grad_input, grad_weight, grad_bias, goff_c, gmask_c, scale,
+                         kh, kw, sh, sw, ph, pw, dh, dw, group, dg)
+    _write_back([(grad_offset, goff_c), (grad_mask, gmask_c)])
+
+
+def _backward_same_dtype(x, weight, offset, mask, grad_output, grad_input, grad_weight, grad_bias, grad_offset, grad_mask,
+                         scale, kh, kw, sh, sw, ph, pw, dh, dw, group, dg):
     B, C, H, W = x.shape
     Cout = weight.size(0)
     Ho, Wo = _out_hw(H, W, kh, kw, sh, sw, ph, pw, dh, dw)
+    offset_in, mask_in = offset, mask
     offset, obs = _slab(offset)
     mbs = gobs = gmbs = 0
     if mask is not None:
@@ -97,8 +177,27 @@ def _backward(x, weight, offset, mask, grad_output, grad_input, grad_weight, gra
         assert grad_mask.size(0) == 0 or grad_mask[0].is_contiguous()
         gmbs = _slab(grad_mask)[1]
     grad_output = grad_output.contiguous()
-    ws, ws_bytes = _workspace(x, C, kh, kw, Ho, Wo, Cout, backward=True)
     p = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    if x.dtype != torch.float32:
+        code, wcode = _codes(x, weight)
+        ws_bytes = _lib.lib().mr_dcn_fused_backward_workspace_bytes_h(B, C, H, W, Cout, Ho, Wo, kh, kw)
+        ws = _half_workspace(x, ws_bytes)
+        with torch.cuda.device(x.device):
+            rc = _lib.lib().mr_dcn_backward_fused_h(
+                x.data_ptr(), weight.data_ptr(), offset.data_ptr(), obs, p(mask), mbs, grad_output.data_ptr(),
+                p(grad_input), p(grad_weight), p(grad_bias), p(grad_offset), gobs, p(grad_mask), gmbs, float(scale),
+                ws.data_ptr(), ws_bytes, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg, code, wcode, _stream())
+        if rc != _lib.MR_ERR_UNSUPPORTED:
+            _lib.check(rc, "dcn_backward")
+            return
+        # outside the fused path: the fp32 kernels on fp32 copies (the accumulating gradients start from the caller's values)
+        grads = (grad_input, grad_weight, grad_bias, grad_offset, grad_mask)
+        g32 = [_float(g) for g in grads]
+        _backward_same_dtype(x.float(), weight.float(), offset_in.float(), _float(mask_in), grad_output.float(), *g32, scale,
+                             kh, kw, sh, sw, ph, pw, dh, dw, group, dg)
+        _write_back([(g, gc) for g, gc in zip(grads, g32) if g is not None])
+        return
+    ws, ws_bytes = _workspace(x, C, kh, kw, Ho, Wo, Cout, backward=True)
     with torch.cuda.device(x.device):
         _lib.check(_lib.lib().mr_dcn_backward_f32(
             x.data_ptr(), weight.data_ptr(), offset.data_ptr(), obs, p(mask), mbs, grad_output.data_ptr(),
