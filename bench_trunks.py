@@ -1,9 +1,13 @@
-"""bench.py --config 3 | 4: the other recognition configurations of BASELINE.json, same JSON contract as the headline line.
+"""bench.py --config 3 | 4 | 5: the other configurations of BASELINE.json, same JSON contract as the headline line;
+benchmarks/db_step.py runs config 6.
 
   config 3   resnet50dilated_ppm + CTCDecoder2D (res50-ppm-2d-ctc.yaml), 3x64x256 lines, feature map 8x32, 2D-CTC loss
   config 4   Resnet50FPN + AttentionDecoder (fpn50-attention-decoder.yaml), 3x64x256 lines (SURVEY.md D3)
+  config 6   deformable_resnet50 + SegDetector(adaptive, k=50) + L1BalanceCELoss (seg_detector_db.yaml), 3x640x640 scenes, per-GPU
+             batch 16, SGD (momentum 0.9, weight decay 1e-4) as in the yaml; the DB tail and loss on csrc/db_head.cu
 
-One "step" = forward + backward + Adam on one synthetic batch (per-GPU batch 32 = BASELINE's 256 over 8 GPUs; --batch overrides).
+One "step" = forward + backward + Adam (config 6: SGD) on one synthetic batch (per-GPU batch 32 = BASELINE's 256 over 8 GPUs;
+config 5: 8, config 6: 16; --batch overrides).
 bf16 compute on the repo's kernels: every convolution of trunk and head runs on the wgmma implicit-GEMM kernels
 (megreader_b200.conv_engine), the 2D-CTC head epilogue + loss on csrc/ctc2d_head.cu + csrc/ctc2d.cu, the attention decoder's recurrent
 loop on csrc/attn_decode.cu, the deformable units on csrc/dcn_tcgen05.cu, BatchNorm on the NHWC row kernels of csrc/nn_kernels.cu;
@@ -25,6 +29,8 @@ CFG = {
     # no EAST yaml exists in the reference; SURVEY.md D4: FeaturePyramid(deformable_resnet50, FPNTopDown) -> EASTDecoder
     5: dict(name="deformable ResNet50 (DCNv2) + FPN + EAST head (SURVEY.md D4 composition)", hw=(512, 512), backbone="deformable_resnet50+FPN",
             decoder="EASTDecoder", l_max=0),
+    6: dict(name="deformable ResNet50 (DCNv2) + DB head + L1BalanceCELoss (seg_detector_db.yaml)", hw=(640, 640),
+            backbone="deformable_resnet50", decoder="SegDetector", l_max=0),
 }
 
 
@@ -62,8 +68,18 @@ def _nbytes(t):
     return t.numel() * t.element_size()
 
 
+def synth_db(seed, n, hw):
+    """seeded images + DB targets (tests/db_data.py: random axis-aligned / rotated text boxes, 5-15 % positive pixels)."""
+    from tests.db_data import db_batch, db_images
+    lab = {k: torch.from_numpy(v) for k, v in db_batch(seed, n, hw[0], hw[1]).items()}
+    return torch.from_numpy(db_images(seed, n, hw[0], hw[1])), lab
+
+
 def make_batch(cfg, seed, n):
     c = CFG[cfg]
+    if cfg == 6:
+        x, lab = synth_db(seed, n, c["hw"])
+        return x, lab, None
     if cfg == 5:
         x, lab = synth_east(seed, n, c["hw"])
         return x, lab, None
@@ -77,7 +93,12 @@ def build(cfg, device, engine=True, wgrad_side_stream=None):
     import decoders
     from tests.weights import fill_state_dict
     c = CFG[cfg]
-    if cfg == 5:
+    if cfg == 6:                         # seg_detector_db.yaml: SegDetectorModel(deformable_resnet50, SegDetector) + L1BalanceCELoss
+        from decoders.seg_detector_loss import L1BalanceCELoss
+        bb = backbones.deformable_resnet50(pretrained=False)
+        dec = decoders.SegDetector(adaptive=True, in_channels=[256, 512, 1024, 2048], k=50)
+        criterion = L1BalanceCELoss()
+    elif cfg == 5:
         from backbones.feature_pyramid import FeaturePyramid
         from backbones.fpn_top_down import FPNTopDown
         bb = FeaturePyramid(backbones.deformable_resnet50(pretrained=False), FPNTopDown([2048, 1024, 512, 256], 256))
@@ -93,6 +114,10 @@ def build(cfg, device, engine=True, wgrad_side_stream=None):
             self.decoder = fill_state_dict(dec, "dec%d." % cfg)
 
         def forward(self, images, targets, lengths):
+            if cfg == 6:                 # structure/model.py:140-155 SegDetectorModel: criterion(decoder(backbone(x)), batch)
+                pred = self.decoder(self.backbone(images), training=True)
+                loss, _ = criterion(pred, targets)
+                return loss, pred
             if cfg == 5:                 # structure/model.py:63-87 DetectionModel: decoder(feature, label, meta, train)
                 loss, pred, _ = self.decoder(self.backbone(images), targets, None, True)
                 return loss, pred
@@ -110,7 +135,7 @@ def conv_roofline(dev, peaks, cfg):
     8x32 map) / the 3x3 512->512 of layer4 at stride-32 resolution (config 4), timed alone with CUDA events."""
     from megreader_b200 import nnops
     N = 256
-    H, W, C, d = (8, 32, 512, 4) if cfg == 3 else ((16, 16, 512, 1) if cfg == 5 else (6, 20, 512, 1))
+    H, W, C, d = (8, 32, 512, 4) if cfg == 3 else ((16, 16, 512, 1) if cfg in (5, 6) else (6, 20, 512, 1))
     x = torch.randn(N, H, W, C, device=dev).bfloat16()
     wm = (torch.randn(C, 9 * C, device=dev) / 68).bfloat16()
     fn = lambda: nnops.conv2d_fprop_tc(x, wm, 3, 3, 1, 1, d, d, d, d)  # noqa: E731
@@ -142,7 +167,7 @@ def cpu_arm(cfg, sample_n, steps, budget_s=25.0):
     c = CFG[cfg]
     cores = max(1, min(32, len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)))
     torch.set_num_threads(cores)
-    if cfg == 5:
+    if cfg in (5, 6):
         return {"value": None, "unit": "lines/s", "cores": cores, "kind": "port",
                 "sample": "not timed: the reference has no CPU implementation of the DCN op (functions/deform_conv.py:40-41 raises)"}
     bb = fill_state_dict(getattr(backbones, c["backbone"])(resnet_pretrained=False), "bb%d." % cfg).train()
@@ -183,13 +208,18 @@ def run(args, peaks, ClockSampler, emit_json):
     if world > 1:
         dist.init_process_group("nccl", device_id=dev)
     torch.manual_seed(0)
-    batch = args.batch or (8 if cfg == 5 else 32)           # BASELINE.json: 256 (cfg 3/4) and 64 (cfg 5) over 8 GPUs
+    batch = args.batch or {5: 8, 6: 16}.get(cfg, 32)        # BASELINE.json: 256 (cfg 3/4) and 64 (cfg 5) over 8 GPUs; yaml: 16 (cfg 6)
     # one GPU: the convolutions' weight gradients run on a side stream (nothing reads a gradient before backward() returns here);
     # N > 1: they accumulate into the flat all-reduce buffer on the backward's stream.  MR_CONV_WGRAD_SIDE_STREAM=0 switches it off.
     side_wgrad = world == 1 and os.environ.get("MR_CONV_WGRAD_SIDE_STREAM", "1") != "0"
     net, n_engine = build(cfg, dev, wgrad_side_stream=side_wgrad)
     params = [p for p in net.parameters() if p.requires_grad]
-    opt = torch.optim.Adam(params, lr=1e-3, fused=True, capturable=True)
+    if cfg == 6:                                             # seg_detector_db.yaml: SGD lr 0.007, momentum 0.9, weight decay 1e-4
+        opt = torch.optim.SGD(params, lr=0.007, momentum=0.9, weight_decay=1e-4)
+        opt_name, opt_desc = "SGD", "SGD lr 0.007 momentum 0.9 weight decay 1e-4"
+    else:
+        opt = torch.optim.Adam(params, lr=1e-3, fused=True, capturable=True)
+        opt_name, opt_desc = "Adam", "Adam lr 1e-3"
     # N > 1: gradients as views of one flat buffer, ONE in-place NCCL all-reduce (AVG) between the two graphs (megreader_b200/dp.py)
     fg = dp.FlatGrads(params) if world > 1 else None
     host = []
@@ -339,14 +369,14 @@ def run(args, peaks, ClockSampler, emit_json):
     ms, ms_e2e = float(t[0]), float(t[1])
     lines = batch * world * args.steps
     out = {
-        "metric": "%s/sec %s train step (fwd+bwd+Adam), %dx%d inputs, batch %d/GPU" % ("scenes" if cfg == 5 else "text-lines", c["name"], c["hw"][0], c["hw"][1], batch),
-        "value": lines / (ms / 1e3), "unit": "scenes/s" if cfg == 5 else "lines/s", "n_gpus": world, "steps": args.steps, "warmup": max(3, args.warmup),
+        "metric": "%s/sec %s train step (fwd+bwd+%s), %dx%d inputs, batch %d/GPU" % ("scenes" if cfg in (5, 6) else "text-lines", c["name"], opt_name, c["hw"][0], c["hw"][1], batch),
+        "value": lines / (ms / 1e3), "unit": "scenes/s" if cfg in (5, 6) else "lines/s", "n_gpus": world, "steps": args.steps, "warmup": max(3, args.warmup),
         "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16",
         "data": "synthetic",
-        "config": {"workload": "%s, 3x%dx%d fp32 input, bf16 compute, Adam lr 1e-3" % (c["name"], c["hw"][0], c["hw"][1]),
+        "config": {"workload": "%s, 3x%dx%d fp32 input, bf16 compute, %s" % (c["name"], c["hw"][0], c["hw"][1], opt_desc),
                    "batch_per_gpu": batch, "global_batch": batch * world, "parallelism": "dp%d" % world,
                    "l2": "3 rotating input batches; weights + gradients + Adam state (> 400 MB) and activations exceed the 50 MB L2"},
-        "e2e": {"value": lines / (ms_e2e / 1e3), "unit": "scenes/s" if cfg == 5 else "lines/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4,
+        "e2e": {"value": lines / (ms_e2e / 1e3), "unit": "scenes/s" if cfg in (5, 6) else "lines/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4,
                 "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": launches_per_step * args.steps, "final_loss": final_loss, "clocks": clocks,
         "engine_convs": n_engine,
@@ -360,11 +390,14 @@ def run(args, peaks, ClockSampler, emit_json):
                          "ReLU / residual add / pooling / interpolation": "library (ATen, channels_last bf16)",
                          "head": ("megreader_b200 fused 2D-CTC epilogue + DP kernels" if cfg == 3 else
                                   "attention decoder: the 32-step loop and its backward through time = megreader_b200 persistent cooperative kernels (csrc/attn_decode.cu), hoisted encoder projection; weight-gradient products over the saved rows: library GEMMs" if cfg == 4 else
+                                  "DB head: convolutions and the 2x2 stride-2 transposed convolutions on the conv engine; sigmoid + step function and "
+                                  "L1BalanceCELoss (hard-negative mining by an on-device radix select) on csrc/db_head.cu; "
+                                  "DCNv2 units: fused wgmma kernels (csrc/dcn_tcgen05.cu)" if cfg == 6 else
                                   "EAST head: 3x3 / 1x1 convolutions and the 2x2 stride-2 transposed convolutions (as 1x1 convolutions + depth-to-space) on the conv engine, losses library; "
                                   "DCNv2 units: fused wgmma forward / weight-gradient / data-gradient kernels (csrc/dcn_tcgen05.cu)"),
                          "conv weight gradients": "side stream, joined at the end of the backward pass (conv_engine.WGRAD_SIDE_STREAM)"
                                                   if side_wgrad else "the backward's stream",
-                         "Adam": "library (torch fused, capturable)", "launch": launch_mode}
+                         opt_name: "library (torch SGD, foreach)" if cfg == 6 else "library (torch fused, capturable)", "launch": launch_mode}
         emit_json(out)
     if world > 1:
         dist.destroy_process_group()

@@ -101,6 +101,38 @@ int mr_ctc2d_head_bwd_f32(const float *mask_logits, const float *cls_logits, con
                           float *grad_cls_logits, float *grad_mask_logits, void *stream);
 
 /* ------------------------------------------------------------------------------------------------
+ * DB (Differentiable Binarization) text-detector tail: SegDetector's sigmoid + step function
+ * (decoders/seg_detector.py:146-147, 189-191) and the L1BalanceCELoss criterion (decoders/seg_detector_loss.py:162-185).
+ * Every entry runs on `stream` and never synchronises with the host, so the whole tail can be captured in a CUDA graph.
+ * ---------------------------------------------------------------------------------------------- */
+/* binary = sigmoid(zb), thresh = sigmoid(zt), thresh_binary = 1 / (1 + exp(-k (binary - thresh))) over n elements, written
+ * as fp32 maps.  zb / zt have dtype 0 = fp32, 1 = bf16, 2 = fp16; compute is fp32.  zt = NULL (adaptive=False): binary only. */
+int mr_db_step_fwd(const void *zb, const void *zt, int dtype, int64_t n, float k, float *binary, float *thresh,
+                   float *thresh_binary, void *stream);
+/* Backward of mr_db_step_fwd from its stored outputs and the incoming map gradients (any may be NULL = zero).  Writes
+ * d_zb (and d_zt unless NULL) in the logits' dtype. */
+int mr_db_step_bwd(const float *binary, const float *thresh, const float *thresh_binary, const float *g_binary,
+                   const float *g_thresh, const float *g_thresh_binary, int dtype, int64_t n, float k, void *d_zb, void *d_zt,
+                   void *stream);
+/* Fused L1BalanceCELoss, fp32.  binary, thresh, thresh_binary, gt: [N,1,H,W]; mask, thresh_map, thresh_mask: [N,H,W].
+ * out_scalars[4] = (loss, bce_loss, dice_loss, l1_loss) with loss = dice + l1_scale * l1 + bce_scale * bce.  The balanced
+ * cross entropy follows the reference's broadcast of gt [N,1,H,W] against mask [N,H,W] (N*N*H*W values, see csrc/db_head.cu)
+ * and its online hard-negative mining: k = min(#negative, int(#positive * negative_ratio)) and the sum of the k largest
+ * negative losses are found on the device by a radix select.  eps is the dice epsilon, bce_eps the one of the cross entropy's
+ * denominator.  Floating-point sums are deterministic.  `workspace` (mr_db_loss_workspace_bytes) keeps the scalars the
+ * backward reads; it must stay untouched in between.  MR_ERR_UNSUPPORTED for N > 192. */
+int64_t mr_db_loss_workspace_bytes(int64_t N, int64_t H, int64_t W);
+int mr_db_loss_fwd_f32(const float *binary, const float *thresh, const float *thresh_binary, const float *gt, const float *mask,
+                       const float *thresh_map, const float *thresh_mask, int N, int H, int W, float eps, float bce_eps,
+                       float l1_scale, float bce_scale, float negative_ratio, void *workspace, float *out_scalars, void *stream);
+/* grad_out[4] (device) = gradients of the four outputs of mr_db_loss_fwd_f32.  Negatives whose loss ties the k-th largest value
+ * each get the weight (k - #above) / #tied. */
+int mr_db_loss_bwd_f32(const float *binary, const float *thresh, const float *thresh_binary, const float *gt, const float *mask,
+                       const float *thresh_map, const float *thresh_mask, int N, int H, int W, float l1_scale, float bce_scale,
+                       const void *workspace, const float *grad_out, float *d_binary, float *d_thresh, float *d_thresh_binary,
+                       void *stream);
+
+/* ------------------------------------------------------------------------------------------------
  * 1D CTC head of the CRNN decoder (replaces the `log_softmax -> nn.CTCLoss(zero_infinity=True)` call,
  * decoders/crnn.py:47-48,95-99; arithmetic restated in decoders/ctc_loss.py:65-122).  fp32.
  * ---------------------------------------------------------------------------------------------- */

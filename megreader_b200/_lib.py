@@ -91,8 +91,14 @@ _SIGS = {
     "mr_dcn_forward_fused_h": [c_p, c_p, c_p, c_p, c_i64, c_p, c_i64, c_p, c_p, c_i64] + [c_int] * 17 + [c_p],
     "mr_dcn_backward_fused_h": [c_p, c_p, c_p, c_i64, c_p, c_i64, c_p, c_p, c_p, c_p, c_p, c_i64, c_p, c_i64, c_f32,
                                 c_p, c_i64] + [c_int] * 17 + [c_p],
+    "mr_db_step_fwd": [c_p, c_p, c_int, c_i64, c_f32, c_p, c_p, c_p, c_p],
+    "mr_db_step_bwd": [c_p] * 6 + [c_int, c_i64, c_f32, c_p, c_p, c_p],
+    "mr_db_loss_workspace_bytes": [c_i64] * 3,
+    "mr_db_loss_fwd_f32": [c_p] * 7 + [c_int] * 3 + [c_f32] * 5 + [c_p, c_p, c_p],
+    "mr_db_loss_bwd_f32": [c_p] * 7 + [c_int] * 3 + [c_f32] * 2 + [c_p] * 6,
 }
 _RESTYPES = {
+    "mr_db_loss_workspace_bytes": c_i64,
     "mr_dcn_fused_workspace_bytes_h": c_i64,
     "mr_dcn_fused_backward_workspace_bytes_h": c_i64,
     "mr_dcn_workspace_bytes": c_i64,
