@@ -72,10 +72,12 @@ struct StateCtx {
     bool active;
     int g, s, b, cur;
     int64_t Tb, L;
-    bool skip_fwd, skip_bwd, in_range;  // in_range: L > 0 && s <= 2L
+    bool skip_fwd, skip_bwd, in_range;  // in_range: (L > 0 || empty_ok) && s <= 2L
 };
+// empty_ok: an empty target keeps its blank-only path (torch's 1D CTC, MODE_FAC_STD).  The 2D op follows the
+// reference's K1/K2, where every state of an L = 0 sample is -inf past t = 0.
 __device__ __forceinline__ StateCtx make_ctx(const Geo &q, int b0, int Gv, const int64_t *tg, const int64_t *il,
-                                             const int64_t *tl) {
+                                             const int64_t *tl, bool empty_ok = false) {
     StateCtx c;
     const int tid = threadIdx.x;
     c.g = tid / q.SS;
@@ -89,7 +91,7 @@ __device__ __forceinline__ StateCtx make_ctx(const Geo &q, int b0, int Gv, const
         c.Tb = il[c.b];
         c.L = tl[c.b];
         if (c.s < 2 * c.L + 1) {
-            c.in_range = c.L > 0;
+            c.in_range = c.L > 0 || empty_ok;
             const int64_t *row = tg + (int64_t)c.b * q.tg_sn;
             if (c.s & 1) {
                 const int64_t me = row[(int64_t)(c.s >> 1) * q.tg_ss];
@@ -467,7 +469,7 @@ __global__ void ctc2d_dp_kernel(Geo q, const real *__restrict__ lp, const int64_
     real *fin = As + 2 * rowStates;                              // [2G] final states, then [G] nll
     unsigned char *pres = reinterpret_cast<unsigned char *>(fin + 3 * q.G);  // [T][G*C]
 
-    const StateCtx c = make_ctx(q, b0, Gv, tg, il, tl);
+    const StateCtx c = make_ctx(q, b0, Gv, tg, il, tl, MODE == MODE_FAC_STD);
     for (int i = tid; i < q.T * rowElems; i += nth) { acc[i] = 0; pres[i] = 0; }
     if (tid < 2 * q.G) fin[tid] = NINF;
 
@@ -610,7 +612,7 @@ __device__ __forceinline__ float warp_sweeps(const WarpDpCtx &w, int lane) {
         const int s = lane * NS + k;
         cur[k] = q.blank; in[k] = skf[k] = skb[k] = false;
         if (s < SS && s < 2 * L + 1) {
-            in[k] = L > 0;
+            in[k] = L > 0 || MODE == MODE_FAC_STD;             // L = 0: the blank-only path of torch's 1D CTC (make_ctx)
             if (s & 1) {
                 const int64_t me = w.row[(int64_t)(s >> 1) * q.tg_ss];
                 cur[k] = clampi(me, q.C);
@@ -1116,7 +1118,7 @@ __device__ __forceinline__ float warp_sweeps4(const Dp4Ctx &w, int lane) {
 }
 
 // lane = column: per-class sums of E[t][s] into the Q row of column t.  cls[j] = class of label j, firstbits bit j = label j
-// is the first label of its class.
+// is the first label of its class; a label of the blank's class has no bit, so it adds to the blank's sum.
 template <int NS>
 __device__ __forceinline__ void collect_transposed(const Dp4Ctx &w, int lane, const int *cls, unsigned firstbits,
                                                    int blank_slot = -1) {
@@ -1209,7 +1211,8 @@ ctc2d_dp4_kernel(Geo q, const float *__restrict__ lp, const int64_t *__restrict_
             lo = __reduce_or_sync(0xffffffffu, lo);
             hi = __reduce_or_sync(0xffffffffu, hi);
             const unsigned same = __match_any_sync(0xffffffffu, myc);
-            const unsigned firstbits = __ballot_sync(0xffffffffu, myc >= 0 && (__ffs(same) - 1) == lane);
+            // a label equal to the blank is not "first": it adds to the blank's sum (K3 sums every state of a class)
+            const unsigned firstbits = __ballot_sync(0xffffffffu, myc >= 0 && myc != q.blank && (__ffs(same) - 1) == lane);
             cls[g * 32 + lane] = myc >= 0 ? myc : 0;
             if (lane == 0) { tmask[2 * g] = lo; tmask[2 * g + 1] = hi; }
             __syncwarp();
@@ -1317,7 +1320,8 @@ ctc2d_dpg_kernel(Geo q, const float *__restrict__ lp, const int64_t *__restrict_
         raw[lane] = r;
         const int myc = lane < L ? (r < 0 ? 0 : (r >= q.C ? q.C - 1 : r)) : -1 - lane;
         const unsigned same = __match_any_sync(0xffffffffu, myc);
-        slot[lane] = 1 + (__ffs(same) - 1);                                 // first label with the same class collects
+        // the first label with the same class collects; a label equal to the blank collects into the blank's slot 0
+        slot[lane] = myc == q.blank ? 0 : 1 + (__ffs(same) - 1);
         clsv[lane] = myc >= 0 ? myc : 0;
     }
     __syncwarp();

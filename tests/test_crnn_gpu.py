@@ -29,9 +29,10 @@ def api():
 def test_ctc1d_vs_reference_call(cuda, zero_inf):
     from megreader_b200 import ctc1d
     rng = np.random.RandomState(0)
-    T, N, C, S = 26, 6, 38, 32
+    T, N, C, S = 26, 7, 38, 32
     logits = torch.from_numpy(rng.standard_normal((T, N, C)).astype(np.float32) * 2)
-    lengths = torch.tensor([3, 8, 1, 12, 5, 30])       # 30 labels in T=26 columns: infeasible -> inf / zero_infinity
+    lengths = torch.tensor([3, 8, 1, 12, 5, 30, 0])    # 30 labels in T=26 columns: infeasible -> inf / zero_infinity;
+    #                                                    0: the blank-only path, nll = -sum_t log p(t, blank) as in torch
     labels = torch.zeros(N, S, dtype=torch.int32)
     for b in range(N):
         labels[b, :lengths[b]] = torch.from_numpy(rng.randint(2, C, size=int(lengths[b])))

@@ -6,7 +6,8 @@ import subprocess
 
 import pytest
 
-from tests import test_conv_tcgen05_gpu, test_dcn_gpu, test_gemm_tcgen05_gpu, test_lstm_step_gpu
+from tests import ctc_variants as cv
+from tests import test_conv_tcgen05_gpu, test_ctc_variants_gpu, test_dcn_gpu, test_gemm_tcgen05_gpu, test_lstm_step_gpu
 from tests import wgmma_variants as wv
 
 
@@ -16,13 +17,16 @@ def so_path():
     return build.build()
 
 
-def compiled_variants(so_path):
+def compiled_kernels(so_path):
     dump = subprocess.run([shutil.which("cuobjdump"), "-symbols", so_path], check=True, capture_output=True,
                           text=True).stdout
     mangled = sorted(set(re.findall(r"\b_Z\w+", dump)))
-    names = subprocess.run([shutil.which("cu++filt")], input="\n".join(mangled), check=True, capture_output=True,
-                           text=True).stdout.splitlines()
-    return {n for n in map(wv.normalise, names) if re.fullmatch(r"\w+_tcgen05_kernel<[\d,]+>", n)}
+    return subprocess.run([shutil.which("cu++filt")], input="\n".join(mangled), check=True, capture_output=True,
+                          text=True).stdout.splitlines()
+
+
+def compiled_variants(so_path):
+    return {n for n in map(wv.normalise, compiled_kernels(so_path)) if re.fullmatch(r"\w+_tcgen05_kernel<[\d,]+>", n)}
 
 
 @pytest.mark.skipif(shutil.which("cuobjdump") is None or shutil.which("cu++filt") is None,
@@ -32,6 +36,63 @@ def test_compiled_instantiations_are_the_known_variants(so_path):
     assert len(wv.ALL_VARIANTS) == 20
     assert found == wv.ALL_VARIANTS, ("not in ALL_VARIANTS: %s; not compiled: %s"
                                       % (sorted(found - wv.ALL_VARIANTS), sorted(wv.ALL_VARIANTS - found)))
+
+
+@pytest.mark.skipif(shutil.which("cuobjdump") is None or shutil.which("cu++filt") is None,
+                    reason="needs cuobjdump and cu++filt from the CUDA toolkit")
+def test_compiled_ctc_instantiations_are_the_known_variants(so_path):
+    """csrc/ctc2d.cu: every compiled ctc2d_* / ctc1d_* / rows_log_softmax kernel is reachable or listed as unreachable"""
+    found = {n for n in map(cv.ctc_normalise, compiled_kernels(so_path))
+             if re.fullmatch(r"(ctc2d_(?!head)\w+|ctc1d_\w+|rows_log_softmax)_kernel(<[\w,]+>)?", n)}
+    assert len(cv.ALL_CTC_VARIANTS) == 70 and len(cv.UNREACHABLE) == 12
+    assert found == cv.CTC_KERNELS, ("unknown: %s; not compiled: %s"
+                                     % (sorted(found - cv.CTC_KERNELS), sorted(cv.CTC_KERNELS - found)))
+
+
+def test_every_ctc_variant_has_a_gpu_case():
+    covered = test_ctc_variants_gpu.VARIANTS
+    assert covered <= cv.ALL_CTC_VARIANTS, sorted(covered - cv.ALL_CTC_VARIANTS)
+    assert covered == cv.ALL_CTC_VARIANTS, "no GPU case expects %s" % sorted(cv.ALL_CTC_VARIANTS - covered)
+
+
+def test_ctc_dispatch_restatement():
+    """spot checks of tests/ctc_variants.py against the host dispatch of csrc/ctc2d.cu (132 SMs, 227 KB opt-in)"""
+    lim = dict(sms=132, smem=232448)
+    p = cv.dp_plan("FAC", 32, 8, 4096, 38, 32, env={}, **lim)
+    assert p == {"kernel": "ctc2d_dp4_kernel<1,8>", "family": "dp4", "G": 8}
+    assert cv.dp_plan("FAC", 32, 8, 32, 38, 32, env={}, **lim)["G"] == 2              # the grid covers the SMs first
+    assert cv.dp_plan("FAC", 32, 8, 4 * 132 + 1, 38, 32, env={}, **lim)["G"] == 4
+    assert cv.dp_plan("FAC", 32, 8, 6 * 132 + 1, 38, 32, env={}, **lim)["G"] == 6
+    assert cv.dp_plan("GRAD", 48, 8, 8 * 132, 38, 32, env={}, **lim)["G"] == 5         # 75 KB plan shrinks an even G
+    assert cv.dp4_pitch(2, 38) == 76 and cv.dp4_pitch(8, 38) == 308
+    assert cv.dp_plan("GRAD", 405, 8, 4, 38, 8, env={}, **lim)["family"] == "dp4"
+    assert cv.dp_plan("GRAD", 406, 8, 4, 38, 8, env={}, **lim)["kernel"] == "ctc2d_dp_warp_kernel<0,1,8>"
+    assert cv.dp_plan("GRAD", 32, 8, 4, 64, 32, env={}, **lim)["family"] == "dp4"
+    assert cv.dp_plan("GRAD", 32, 8, 4, 65, 32, env={}, **lim)["kernel"] == "ctc2d_dpg_kernel<0>"
+    assert cv.dp_plan("GRAD", 32, 8, 4, 38, 33, env={}, **lim)["kernel"] == "ctc2d_dp_warp_kernel<0,3,8>"
+    assert cv.dp_plan("FAC", 32, 2, 4, 38, 16, env={"MR_CTC2D_DP_V3": "1"}, **lim)["kernel"] == \
+        "ctc2d_dp_warp_kernel<1,2,0>"
+    assert cv.dp_plan("FAC", 32, 8, 4, 38, 16, env={"MR_CTC2D_BLOCK_DP": "1"}, **lim)["kernel"] == \
+        "ctc2d_dp_kernel<float,true,1,8>"
+    assert cv.dp_plan("FAC_STD", 65, 1, 512, 38, 32, env={}, **lim) == {
+        "kernel": "ctc2d_dp_warp_kernel<2,3,0>", "family": "dp_warp", "G": 4, "NSMAX": 3}
+    assert cv.dp_plan("FAC_STD", 65, 1, 512, 38, 32, fast=False, env={}, **lim)["kernel"] == "ctc2d_dp_kernel<float,false,2,0>"
+    assert cv.dp_plan("GRAD", 16, 8, 4, 38, 32, real="double", env={}, **lim)["kernel"] == "ctc2d_dp_kernel<double,false,0,8>"
+    w = cv.dp_plan("GRAD", 12, 8, 4, 38, 256, env={}, **lim)
+    assert w["kernel"] == "ctc2d_dp_warp_kernel<0,32,8>" and w["G"] == 4
+    assert cv.sample_sweeps(w, 256, [0, 15, 16, 31, 32, 47, 48, 63, 64, 127, 128, 255, 256]) == [
+        "warp_sweeps<%d>" % n for n in (1, 1, 2, 2, 3, 3, 4, 4, 8, 8, 16, 16, 32)]
+    assert cv.sample_sweeps(p, 32, [0, 15, 16, 31, 32]) == ["warp_sweeps4<%d>" % n for n in (1, 1, 2, 2, 3)]
+    assert cv.dp4_rounds(p, 32, [32, 32, 32, 1, 0, 5, 5, 5]) == [2]                     # 3+3+3 slots > 8: a second round
+    assert cv.alpha_variant(32, 8, 38, 32, smem=232448) == "ctc2d_alpha_kernel<float,true,true,8>"
+    assert cv.alpha_variant(6, 4, 4001, 3, smem=232448) == "ctc2d_alpha_kernel<float,true,false,0>"
+    assert cv.alpha_variant(6, 8, 1000, 3, real="double", smem=232448) == "ctc2d_alpha_kernel<double,false,false,0>"
+    assert cv.apply_variant(8, 6, 38) == "ctc2d_apply_kernel<true,4,8>"
+    assert cv.apply_variant(8, 7, 38) == "ctc2d_apply_kernel<true,1,0>"
+    assert cv.apply_variant(3, 4, 7, fast=False, aligned=False) == "ctc2d_apply_kernel<false,1,0>"
+    assert cv.ctc_normalise("void <unnamed>::ctc2d_dp_kernel<float, (bool)1, (int)2, (int)0>(<unnamed>::Geo, const T1 *)") \
+        == "ctc2d_dp_kernel<float,true,2,0>"
+    assert cv.ctc_normalise("<unnamed>::rows_log_softmax_kernel(const float *, long, int, float *)") == "rows_log_softmax_kernel"
 
 
 def test_every_variant_has_a_gpu_case():
