@@ -28,6 +28,11 @@
 // fp32 and each column value is rounded ONCE to T, so there is one operand (no hi / lo split) and one MMA per K block
 // (.f32.f16.f16 or .f32.bf16.bf16), still accumulated in fp32.  The fp32 kernels keep their names and code: their __global__
 // functions are thin wrappers around the T = float instantiation of the shared __device__ bodies.
+//
+// The host side is one path for every T as well: dcn_shape() decides whether a call is fused (and is the only reader of the
+// MR_DCN_UNFUSED* switches), DcnWs lays out the workspace, and dcn_forward<T, WT> / dcn_backward<T, WT> run the pre-passes (NHWC
+// copy, weight pack, grad_output re-tile: hi / lo for fp32, one T copy otherwise), the fused kernels and the post-passes.  The
+// C entry points below only check their arguments and call them.
 #include "wgmma.cuh"
 #include <math.h>
 #include <stdlib.h>
@@ -79,7 +84,6 @@ template <typename T> struct DcnFArgsT {
     int B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, Ho, Wo, P;
     int tiles_per_sample, tiles_x, ncb, nkb;     // 8 x 16 pixel tiles; ncb = C / 64 channel blocks, nkb = kh*kw*ncb K blocks
 };
-struct DcnFArgs : DcnFArgsT<float> {};
 
 // OPS = 2: fp32 input (hi and lo of both operands), 1: half precision
 template <int BN, int STAGES, int OPS = 2>
@@ -324,7 +328,7 @@ __device__ __forceinline__ void dcn_fwd_body(const CUtensorMap &tmWh, const CUte
 
 template <int BN, int STAGES>
 __global__ void __launch_bounds__(kDcnThreads, 1)
-dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, DcnFArgs a) {
+dcn_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, DcnFArgsT<float> a) {
     dcn_fwd_body<float, BN, STAGES>(tmWh, tmWl, a);
 }
 
@@ -353,7 +357,6 @@ template <typename T> struct DcnWArgsT {
     int B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, Ho, Wo, P;
     int tiles_per_sample, tiles_x, ncb, nkb, ntiles, splits;
 };
-struct DcnWArgs : DcnWArgsT<float> {};
 
 template <int OPS>
 struct DcnWSmemT {
@@ -365,7 +368,6 @@ struct DcnWSmemT {
     static constexpr int TAP_OFF = BAR_OFF + 128;
     static constexpr int TOTAL = TAP_OFF + 2 * BM * 24 + 1024;   // one tap-table row set per tile parity
 };
-typedef DcnWSmemT<2> DcnWSmem;
 
 template <typename T>
 __device__ __forceinline__ void dcn_wgrad_body(const CUtensorMap &tmGh, const CUtensorMap &tmGl, const DcnWArgsT<T> &a) {
@@ -574,7 +576,7 @@ __device__ __forceinline__ void dcn_wgrad_body(const CUtensorMap &tmGh, const CU
 }
 
 __global__ void __launch_bounds__(kDcnThreads, 1)
-dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_constant__ CUtensorMap tmGl, DcnWArgs a) {
+dcn_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_constant__ CUtensorMap tmGl, DcnWArgsT<float> a) {
     dcn_wgrad_body<float>(tmGh, tmGl, a);
 }
 
@@ -607,7 +609,6 @@ template <typename T> struct DcnDArgsT {
     int B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, Ho, Wo, P;
     int tiles_per_sample, tiles_x, nch, nkk, tap_splits;     // nch = C / 128 channel chunks, nkk = Cout / 32 K blocks
 };
-struct DcnDArgs : DcnDArgsT<float> {};
 
 template <int OPS>
 struct DcnDSmemT {
@@ -624,7 +625,6 @@ struct DcnDSmemT {
     static constexpr int TAB_BYTES = 2 * BM * (3 * 16 + 8 + 4);          // tap tables, double-buffered by tap parity
     static constexpr int TOTAL = TAB_OFF + TAB_BYTES + 1024;
 };
-typedef DcnDSmemT<2> DcnDSmem;
 
 __device__ __forceinline__ void red_add_v4(float *p, float a, float b, float c, float d) {
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
@@ -899,7 +899,7 @@ __device__ __forceinline__ void dcn_dgrad_body(const CUtensorMap &tmGh, const CU
 
 __global__ void __launch_bounds__(kDcnThreads, 1)
 dcn_dgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmGh, const __grid_constant__ CUtensorMap tmGl,
-                         const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, DcnDArgs a) {
+                         const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, DcnDArgsT<float> a) {
     dcn_dgrad_body<float>(tmGh, tmGl, tmWh, tmWl, a);
 }
 
@@ -909,10 +909,35 @@ dcn_dgrad_half_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_cons
     dcn_dgrad_body<T>(tmG, tmG, tmW, tmW, a);
 }
 
+// ---------------------------------------------------------------- pre- and post-passes (T = float, __half or bf16)
+// The MMA operands they produce are DcnElem<T>::kOps copies: bf16 hi and lo for T = float, one T copy otherwise (`lo` is then not
+// written).
+
+// x [B][C][P] -> y [B][P][C] (exact), 32 x 32 tiles through shared memory
+template <typename T>
+__global__ void __launch_bounds__(256) dcn_nchw_to_nhwc_kernel(const T *__restrict__ x, T *__restrict__ y, int C, int P) {
+    __shared__ float tile[32][33];
+    const int b = blockIdx.z, c0 = blockIdx.y * 32, p0 = blockIdx.x * 32;
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    const T *xb = x + (int64_t)b * C * P;
+    T *yb = y + (int64_t)b * C * P;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int c = c0 + ty + 8 * j, p = p0 + tx;
+        tile[ty + 8 * j][tx] = (c < C && p < P) ? ld1(xb + (int64_t)c * P + p) : 0.f;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const int p = p0 + ty + 8 * j, c = c0 + tx;
+        if (p < P && c < C) yb[(int64_t)p * C + c] = from_f32<T>(tile[tx][ty + 8 * j]);
+    }
+}
+
 // y [B][C][P] += x [B][P][C]   (the NHWC gradient scratch folded into the caller's NCHW grad_input, which is accumulated into;
 // a T grad_input is rounded once, after the fp32 sum)
 template <typename T>
-__device__ __forceinline__ void nhwc_to_nchw_add_body(const float *__restrict__ x, T *__restrict__ y, int C, int P) {
+__global__ void __launch_bounds__(256) dcn_nhwc_to_nchw_add_kernel(const float *__restrict__ x, T *__restrict__ y, int C, int P) {
     __shared__ float t[32][33];
     const int b = blockIdx.z, p0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
     const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
@@ -929,22 +954,15 @@ __device__ __forceinline__ void nhwc_to_nchw_add_body(const float *__restrict__ 
         }
     }
 }
-__global__ void __launch_bounds__(256) dcn_nhwc_to_nchw_add_kernel(const float *__restrict__ x, float *__restrict__ y, int C, int P) {
-    nhwc_to_nchw_add_body<float>(x, y, C, P);
-}
-template <typename T>
-__global__ void __launch_bounds__(256) dcn_nhwc_to_nchw_add_half_kernel(const float *__restrict__ x, T *__restrict__ y, int C, int P) {
-    nhwc_to_nchw_add_body<T>(x, y, C, P);
-}
 
-// grad_output [B][Cout][P] T -> [B * tiles][Cout][128] T in the 8 x 16 tile order of the kernels (0 outside the map): the single
-// MMA operand of the half-precision gradient kernels
+// grad_output [B][Cout][P] T -> [B * tiles][Cout][128] in the 8 x 16 tile order of the kernels (0 outside the map)
 template <typename T>
-__global__ void dcn_go_retile_half_kernel(const T *__restrict__ go, int B, int Cout, int Ho, int Wo, int tiles_x, int tiles_per_sample,
-                                          T *__restrict__ out) {
-    // one thread = one 16-pixel tile row of one channel: 32 contiguous bytes in and out
+__global__ void dcn_go_retile_kernel(const T *__restrict__ go, int B, int Cout, int Ho, int Wo, int tiles_x, int tiles_per_sample,
+                                     typename DcnElem<T>::Mma *__restrict__ hi, typename DcnElem<T>::Mma *__restrict__ lo) {
+    // one thread = one 16-pixel tile row of one channel: 16 contiguous elements in, 32 contiguous bytes out per copy
+    constexpr int kVecs = sizeof(T);                                    // 16-byte vectors per row
     const int64_t n = (int64_t)B * tiles_per_sample * Cout * 8;
-    const bool vec = (Wo & 7) == 0 && ((uintptr_t)go & 15) == 0;     // 16-byte rows (a caller's view may start anywhere)
+    const bool vec = (Wo * (int)sizeof(T)) % 16 == 0 && ((uintptr_t)go & 15) == 0;     // 16-byte rows (a caller's view may start anywhere)
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const int gr = (int)(i & 7);
         int64_t t = i >> 3;
@@ -953,23 +971,39 @@ __global__ void dcn_go_retile_half_kernel(const T *__restrict__ go, int B, int C
         const int b = (int)(t / tiles_per_sample);
         const int py = (tile / tiles_x) * 8 + gr, px0 = (tile % tiles_x) * 16;
         const T *src = go + ((int64_t)b * Cout + co) * Ho * Wo + (int64_t)py * Wo + px0;
-        uint4 *dst = reinterpret_cast<uint4 *>(out + i * 16);
+        uint4 u[kVecs];
+        T *v = reinterpret_cast<T *>(u);
         if (py < Ho && vec && px0 + 16 <= Wo) {
-            dst[0] = __ldg(reinterpret_cast<const uint4 *>(src));
-            dst[1] = __ldg(reinterpret_cast<const uint4 *>(src) + 1);
-        } else {
-            uint4 v[2];
-            T *h = reinterpret_cast<T *>(v);
 #pragma unroll
-            for (int e = 0; e < 16; ++e) h[e] = (py < Ho && px0 + e < Wo) ? src[e] : from_f32<T>(0.f);
-            dst[0] = v[0]; dst[1] = v[1];
+            for (int e = 0; e < kVecs; ++e) u[e] = __ldg(reinterpret_cast<const uint4 *>(src) + e);
+        } else {
+#pragma unroll
+            for (int e = 0; e < 16; ++e) v[e] = (py < Ho && px0 + e < Wo) ? src[e] : from_f32<T>(0.f);
+        }
+        uint4 *dh = reinterpret_cast<uint4 *>(hi + i * 16);
+        if constexpr (DcnElem<T>::kSplit) {
+            uint32_t ph[8], pl[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const __nv_bfloat162 h2 = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
+                const float2 f = __bfloat1622float2(h2);
+                const __nv_bfloat162 l2 = __floats2bfloat162_rn(v[2 * e] - f.x, v[2 * e + 1] - f.y);
+                ph[e] = *reinterpret_cast<const uint32_t *>(&h2);
+                pl[e] = *reinterpret_cast<const uint32_t *>(&l2);
+            }
+            uint4 *dl = reinterpret_cast<uint4 *>(lo + i * 16);
+            dh[0] = make_uint4(ph[0], ph[1], ph[2], ph[3]); dh[1] = make_uint4(ph[4], ph[5], ph[6], ph[7]);
+            dl[0] = make_uint4(pl[0], pl[1], pl[2], pl[3]); dl[1] = make_uint4(pl[4], pl[5], pl[6], pl[7]);
+        } else {
+            dh[0] = u[0]; dh[1] = u[1];
         }
     }
 }
 
-// weight [Cout][C][K] WT (fp32 or T) -> T [Cout][(cb * K + k) * 64 + cl]  (channel c = cb * 64 + cl), the layout of dcn_weight_pack_kernel
+// weight [Cout][C][K] WT (fp32 or T) -> [Cout][(cb * K + k) * 64 + cl]  (channel c = cb * 64 + cl)
 template <typename WT, typename T>
-__global__ void dcn_weight_pack_half_kernel(const WT *__restrict__ w, int Cout, int C, int K, T *__restrict__ out) {
+__global__ void dcn_weight_pack_kernel(const WT *__restrict__ w, int Cout, int C, int K, typename DcnElem<T>::Mma *__restrict__ hi,
+                                       typename DcnElem<T>::Mma *__restrict__ lo) {
     const int64_t n = (int64_t)Cout * C * K;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const int cl = (int)(i % 64);
@@ -977,7 +1011,14 @@ __global__ void dcn_weight_pack_half_kernel(const WT *__restrict__ w, int Cout, 
         const int k = (int)(t % K); t /= K;
         const int cb = (int)(t % (C / 64));
         const int co = (int)(t / (C / 64));
-        out[i] = from_f32<T>(to_f32(w[((int64_t)co * C + cb * 64 + cl) * K + k]));
+        const float v = to_f32(w[((int64_t)co * C + cb * 64 + cl) * K + k]);
+        if constexpr (DcnElem<T>::kSplit) {
+            const bf16 h = __float2bfloat16_rn(v);
+            hi[i] = h;
+            lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
+        } else {
+            hi[i] = from_f32<T>(v);
+        }
     }
 }
 
@@ -1010,94 +1051,6 @@ __global__ void __launch_bounds__(256) dcn_bias_grad_half_kernel(const T *__rest
     }
 }
 
-// grad_output [B][Cout][P] fp32 -> hi / lo bf16 [B * tiles][Cout][128] in the 8 x 16 tile order of the kernels (0 outside the map)
-__global__ void dcn_go_retile_kernel(const float *__restrict__ go, int B, int Cout, int Ho, int Wo, int tiles_x, int tiles_per_sample,
-                                     bf16 *__restrict__ hi, bf16 *__restrict__ lo) {
-    // one thread = one 16-pixel tile row of one channel: 64 contiguous bytes in, 32 + 32 contiguous bytes out
-    const int64_t n = (int64_t)B * tiles_per_sample * Cout * 8;
-    const bool vec = (Wo & 3) == 0;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        const int gr = (int)(i & 7);
-        int64_t t = i >> 3;
-        const int co = (int)(t % Cout); t /= Cout;
-        const int tile = (int)(t % tiles_per_sample);
-        const int b = (int)(t / tiles_per_sample);
-        const int py = (tile / tiles_x) * 8 + gr, px0 = (tile % tiles_x) * 16;
-        float v[16];
-        const float *src = go + ((int64_t)b * Cout + co) * Ho * Wo + (int64_t)py * Wo + px0;
-        if (py < Ho && vec && px0 + 16 <= Wo) {
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float4 f = __ldg(reinterpret_cast<const float4 *>(src) + e);
-                v[4 * e] = f.x; v[4 * e + 1] = f.y; v[4 * e + 2] = f.z; v[4 * e + 3] = f.w;
-            }
-        } else {
-#pragma unroll
-            for (int e = 0; e < 16; ++e) v[e] = (py < Ho && px0 + e < Wo) ? __ldg(src + e) : 0.f;
-        }
-        uint32_t ph[8], pl[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-            const __nv_bfloat162 h2 = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
-            const float2 f = __bfloat1622float2(h2);
-            const __nv_bfloat162 l2 = __floats2bfloat162_rn(v[2 * e] - f.x, v[2 * e + 1] - f.y);
-            ph[e] = *reinterpret_cast<const uint32_t *>(&h2);
-            pl[e] = *reinterpret_cast<const uint32_t *>(&l2);
-        }
-        uint4 *dh = reinterpret_cast<uint4 *>(hi + i * 16), *dl = reinterpret_cast<uint4 *>(lo + i * 16);
-        dh[0] = make_uint4(ph[0], ph[1], ph[2], ph[3]); dh[1] = make_uint4(ph[4], ph[5], ph[6], ph[7]);
-        dl[0] = make_uint4(pl[0], pl[1], pl[2], pl[3]); dl[1] = make_uint4(pl[4], pl[5], pl[6], pl[7]);
-    }
-}
-
-// x [B][C][P] -> y [B][P][C] (fp32 or T, exact), 32 x 32 tiles through shared memory
-template <typename T>
-__device__ __forceinline__ void nchw_to_nhwc_body(const T *__restrict__ x, T *__restrict__ y, int C, int P) {
-    __shared__ float tile[32][33];
-    const int b = blockIdx.z, c0 = blockIdx.y * 32, p0 = blockIdx.x * 32;
-    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-    const T *xb = x + (int64_t)b * C * P;
-    T *yb = y + (int64_t)b * C * P;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int c = c0 + ty + 8 * j, p = p0 + tx;
-        tile[ty + 8 * j][tx] = (c < C && p < P) ? ld1(xb + (int64_t)c * P + p) : 0.f;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const int p = p0 + ty + 8 * j, c = c0 + tx;
-        if (p < P && c < C) yb[(int64_t)p * C + c] = from_f32<T>(tile[tx][ty + 8 * j]);
-    }
-}
-__global__ void __launch_bounds__(256)
-dcn_nchw_to_nhwc_kernel(const float *__restrict__ x, float *__restrict__ y, int C, int P) {
-    nchw_to_nhwc_body<float>(x, y, C, P);
-}
-template <typename T>
-__global__ void __launch_bounds__(256)
-dcn_nchw_to_nhwc_half_kernel(const T *__restrict__ x, T *__restrict__ y, int C, int P) {
-    nchw_to_nhwc_body<T>(x, y, C, P);
-}
-
-// weight [Cout][C][K] fp32 -> hi / lo bf16 [Cout][(cb * K + k) * 64 + cl]  (channel c = cb * 64 + cl)
-__global__ void dcn_weight_pack_kernel(const float *__restrict__ w, int Cout, int C, int K, bf16 *__restrict__ hi, bf16 *__restrict__ lo) {
-    const int64_t n = (int64_t)Cout * C * K;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        // i = co * (C*K) + (cb * K + k) * 64 + cl   with channel c = cb * 64 + cl
-        const int cl = (int)(i % 64);
-        int64_t t = i / 64;
-        const int k = (int)(t % K); t /= K;
-        const int cb = (int)(t % (C / 64));
-        const int co = (int)(t / (C / 64));
-        const int c = cb * 64 + cl;
-        const float v = w[((int64_t)co * C + c) * K + k];
-        const bf16 h = __float2bfloat16_rn(v);
-        hi[i] = h;
-        lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-    }
-}
-
 // split-K of the fused weight gradient over the pixel tiles: whole waves of CTAs (one CTA per SM), the fewest
 // (rounds x tiles per CTA + per-CTA overhead)
 int dcn_wgrad_splits(int nkb, int Cout, int ntiles) {
@@ -1127,198 +1080,209 @@ int dcn_dgrad_tap_splits(int K, int ntiles, int nch) {
     return splits;
 }
 
-// launch of the fused weight gradient once the NHWC input and the re-tiled grad_output exist
-int launch_dcn_wgrad(DcnWArgs &a, const bf16 *ghi, const bf16 *glo, cudaStream_t st) {
-    CUtensorMap th, tl;
-    int rc = make_map(&th, ghi, BM, (int64_t)a.ntiles * a.Cout, BM, BK, BM);
-    if (rc) return rc;
-    rc = make_map(&tl, glo, BM, (int64_t)a.ntiles * a.Cout, BM, BK, BM);
-    if (rc) return rc;
-    const int splits = dcn_wgrad_splits(a.nkb, a.Cout, a.ntiles);
-    a.splits = splits;
-    { int rc_attr = ensure_dyn_smem((const void *)dcn_wgrad_tcgen05_kernel, DcnWSmem::TOTAL, "dcn_wgrad_tcgen05 smem attr"); if (rc_attr) return rc_attr; }
-    dim3 grid((unsigned)a.nkb, (unsigned)splits, (unsigned)(a.Cout / BM));
-    dcn_wgrad_tcgen05_kernel<<<grid, kDcnThreads, DcnWSmem::TOTAL, st>>>(th, tl, a);
-    return check_launch("dcn_wgrad_tcgen05_kernel");
-}
-
-template <int BN, int STAGES>
-int launch_dcn_fwd(const CUtensorMap &th, const CUtensorMap &tl, const DcnFArgs &a, cudaStream_t st) {
-    using L = DcnSmem<BN, STAGES>;
-    auto kern = dcn_fwd_tcgen05_kernel<BN, STAGES>;
-    const int smem = L::total(a.kh * a.kw);
-    if (smem > 227 * 1024) return MR_ERR_UNSUPPORTED;
-    { int rc_attr = ensure_dyn_smem((const void *)kern, smem, "dcn_fwd_tcgen05 smem attr"); if (rc_attr) return rc_attr; }
-    dim3 grid((unsigned)(a.B * a.tiles_per_sample), (unsigned)(a.Cout / BN), 1);
-    kern<<<grid, kDcnThreads, smem, st>>>(th, tl, a);
-    return check_launch("dcn_fwd_tcgen05_kernel");
-}
-
-// ---------------------------------------------------------------- half precision (T = __half / bf16, weights WT = float or T)
-// Workspace pieces, each 256-byte aligned.  Forward: NHWC T input, packed T weights, fp32 bias.  Backward: NHWC T input, fp32 NHWC
-// grad_input scratch, re-tiled T grad_output, packed T weights, fp32 grad_weight scratch (used when WT = T).
-struct DcnHalfWs {
-    int64_t x, gx, g, w, gw, bias;
-    DcnHalfWs(int64_t B, int64_t C, int64_t H, int64_t W, int64_t Cout, int64_t Ho, int64_t Wo, int64_t kh, int64_t kw) {
-        const int64_t tiles = ceil_div(Wo, 16) * ceil_div(Ho, 8);
-        x = round_up(B * H * W * C * 2, 256);
-        gx = round_up(B * H * W * C * 4, 256);
-        g = round_up(B * tiles * Cout * BM * 2, 256);
-        w = round_up(Cout * C * kh * kw * 2, 256);
-        gw = round_up(Cout * C * kh * kw * 4, 256);
-        bias = round_up(Cout * 4, 256);
-    }
-    int64_t forward() const { return x + w + bias; }
-    int64_t backward() const { return x + gx + g + w + gw; }
+// ---------------------------------------------------------------- host path, one for every element type
+// The shape of a fused call: the C-ABI arguments and the 8 x 16 output-pixel tiles.
+struct DcnShape {
+    int B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw;
+    int Ho, Wo, P, tiles_x, tiles_per_sample, ntiles;
 };
 
-inline unsigned grid_cap(int64_t n, int per_sm) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), (int64_t)sm_count() * per_sm)); }
+// what a call runs, for dcn_shape()
+enum { kFwd = 1, kWgrad = 2, kDgrad = 4 };
 
+// Fills s and says whether the fused kernels of element type T take the call: MR_ERR_UNSUPPORTED (the caller then uses dcn.cu)
+// or MR_ERR_BAD_SHAPE before any work.  The only reader of the MR_DCN_UNFUSED* switches.
 template <typename T>
-int dcn_to_nhwc_half(const T *input, T *xh, int B, int C, int H, int W, cudaStream_t st) {
-    dim3 tg((unsigned)ceil_div((int64_t)H * W, 32), (unsigned)ceil_div(C, 32), (unsigned)B);
-    dcn_nchw_to_nhwc_half_kernel<T><<<tg, 256, 0, st>>>(input, xh, C, H * W);
-    return check_launch("dcn_nchw_to_nhwc_half_kernel");
+int dcn_shape(DcnShape &s, int B, int C, int H, int W, int Cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw,
+              int group, int dg, int parts) {
+    if (group != 1 || dg != 1 || C % 64 || Cout % 128 || B <= 0 || H > 65535 || W > 65535) return MR_ERR_UNSUPPORTED;
+    if (getenv("MR_DCN_UNFUSED")) return MR_ERR_UNSUPPORTED;
+    if (kh <= 0 || kw <= 0 || sh <= 0 || sw <= 0 || dh <= 0 || dw <= 0 || ph < 0 || pw < 0 || C <= 0 || H <= 0 || W <= 0) return MR_ERR_BAD_SHAPE;
+    s = DcnShape{B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw};
+    s.Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1;
+    s.Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
+    if (s.Ho <= 0 || s.Wo <= 0) return MR_ERR_BAD_SHAPE;
+    s.P = s.Ho * s.Wo;
+    s.tiles_x = (int)ceil_div(s.Wo, 16);
+    s.tiles_per_sample = s.tiles_x * (int)ceil_div(s.Ho, 8);
+    if ((int64_t)B * s.tiles_per_sample * Cout > 0x7fffffffLL) return MR_ERR_UNSUPPORTED;    // TMA rows of the re-tiled grad_output
+    s.ntiles = B * s.tiles_per_sample;
+    if ((parts & kFwd) && DcnSmem<128, 2, DcnElem<T>::kOps>::total(kh * kw) > 227 * 1024) return MR_ERR_UNSUPPORTED;
+    if ((parts & kWgrad) && getenv("MR_DCN_UNFUSED_WGRAD")) return MR_ERR_UNSUPPORTED;
+    if ((parts & kDgrad) && (C % 128 || getenv("MR_DCN_UNFUSED_DGRAD"))) return MR_ERR_UNSUPPORTED;
+    return MR_OK;
 }
 
-template <typename T, typename WT>
-int dcn_pack_weight_half(const WT *weight, T *wp, int Cout, int C, int K, cudaStream_t st) {
-    const int64_t nw = (int64_t)Cout * C * K;
-    dcn_weight_pack_half_kernel<WT, T><<<grid_cap(nw, 8), 256, 0, st>>>(weight, Cout, C, K, wp);
-    return check_launch("dcn_weight_pack_half_kernel");
-}
-
-template <typename T, typename WT>
-int dcn_forward_half(const T *input, const WT *weight, const WT *bias, const T *offset, int64_t offset_bstride, const T *mask,
-                     int64_t mask_bstride, T *output, unsigned char *ws, int B, int C, int H, int W, int Cout, int kh, int kw, int sh,
-                     int sw, int ph, int pw, int dh, int dw, cudaStream_t st) {
-    DcnFArgsT<T> a;
-    a.B = B; a.C = C; a.H = H; a.W = W; a.Cout = Cout; a.kh = kh; a.kw = kw; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw;
-    a.dh = dh; a.dw = dw;
-    a.Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1;
-    a.Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
-    a.P = a.Ho * a.Wo;
-    a.tiles_x = (int)ceil_div(a.Wo, 16);
-    a.tiles_per_sample = a.tiles_x * (int)ceil_div(a.Ho, 8);
-    a.ncb = C / BK; a.nkb = kh * kw * a.ncb;
-    const DcnHalfWs L(B, C, H, W, Cout, a.Ho, a.Wo, kh, kw);
-    T *xh = (T *)ws, *wp = (T *)(ws + L.x);
-    float *bf = (float *)(ws + L.x + L.w);
-    int rc = dcn_to_nhwc_half(input, xh, B, C, H, W, st);
-    if (rc) return rc;
-    if ((rc = dcn_pack_weight_half(weight, wp, Cout, C, kh * kw, st))) return rc;
-    const float *b32 = nullptr;
-    if constexpr (std::is_same<WT, float>::value) {
-        b32 = bias;
-        (void)bf;
-    } else if (bias) {
-        dcn_to_f32_kernel<WT><<<1, 256, 0, st>>>(bias, bf, Cout);
-        if ((rc = check_launch("dcn_to_f32_kernel"))) return rc;
-        b32 = bf;
+// The caller's workspace in 256-byte pieces: x = NHWC T input, g = re-tiled grad_output and w = packed weights (kOps copies
+// each), gx = fp32 NHWC grad_input scratch, and for half precision bias = fp32 bias (T bias) and gw = fp32 grad_weight scratch
+// (T grad_weight).  Forward: x | w | bias.  Backward: x | g | w | gx | gw, so a weight gradient alone needs only x | g.
+template <typename T> struct DcnWs {
+    static constexpr int kOps = DcnElem<T>::kOps;
+    static constexpr bool kHalf = !DcnElem<T>::kSplit;
+    int64_t x, g, w, gx, gw, bias;
+    DcnWs(int64_t B, int64_t C, int64_t H, int64_t W, int64_t Cout, int64_t Ho, int64_t Wo, int64_t kh, int64_t kw) {
+        x = round_up(B * H * W * C * (int64_t)sizeof(T), 256);
+        g = round_up(B * ceil_div(Wo, 16) * ceil_div(Ho, 8) * Cout * BM * 2, 256);
+        w = round_up(Cout * C * kh * kw * 2, 256);
+        gx = round_up(B * H * W * C * 4, 256);
+        gw = kHalf ? round_up(Cout * C * kh * kw * 4, 256) : 0;
+        bias = kHalf ? round_up(Cout * 4, 256) : 0;
     }
-    a.xh = xh; a.off = offset; a.msk = mask; a.bias = b32; a.out = output; a.off_bs = offset_bstride; a.mask_bs = mask_bstride;
-    CUtensorMap tw;
-    const int64_t Kt = (int64_t)kh * kw * C;
-    if ((rc = make_map(&tw, wp, Kt, Cout, Kt, BK, 128))) return rc;      // 2-byte elements: the bf16 map type only sets the size
-    const int smem = DcnSmem<128, 2, 1>::total(kh * kw);
-    if (smem > 227 * 1024) return MR_ERR_UNSUPPORTED;
-    { int rc_attr = ensure_dyn_smem((const void *)dcn_fwd_half_kernel<T>, smem, "dcn_fwd_half smem attr"); if (rc_attr) return rc_attr; }
-    dim3 grid((unsigned)(a.B * a.tiles_per_sample), (unsigned)(a.Cout / 128), 1);
-    dcn_fwd_half_kernel<T><<<grid, kDcnThreads, smem, st>>>(tw, a);
-    return check_launch("dcn_fwd_half_kernel");
+    explicit DcnWs(const DcnShape &s) : DcnWs(s.B, s.C, s.H, s.W, s.Cout, s.Ho, s.Wo, s.kh, s.kw) {}
+    // byte offsets
+    int64_t fwd_bias() const { return x + kOps * w; }
+    int64_t bwd_w() const { return x + kOps * g; }
+    int64_t bwd_gx() const { return bwd_w() + kOps * w; }
+    int64_t bwd_gw() const { return bwd_gx() + gx; }
+    // sizes
+    int64_t forward() const { return fwd_bias() + bias; }
+    int64_t wgrad() const { return bwd_w(); }
+    int64_t backward() const { return bwd_gw() + gw; }
+};
+
+// the shape fields every kernel argument struct carries
+template <typename A> void set_shape(A &a, const DcnShape &s) {
+    a.B = s.B; a.C = s.C; a.H = s.H; a.W = s.W; a.Cout = s.Cout; a.kh = s.kh; a.kw = s.kw; a.sh = s.sh; a.sw = s.sw; a.ph = s.ph;
+    a.pw = s.pw; a.dh = s.dh; a.dw = s.dw; a.Ho = s.Ho; a.Wo = s.Wo; a.P = s.P; a.tiles_per_sample = s.tiles_per_sample;
+    a.tiles_x = s.tiles_x;
 }
 
+inline unsigned grid_cap(int64_t n, int per_sm) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, 256), (int64_t)sm_count() * per_sm)); }
+// the 32 x 32 (pixel, channel) tiles of the NCHW <-> NHWC passes
+inline dim3 transpose_grid(const DcnShape &s) { return dim3((unsigned)ceil_div((int64_t)s.H * s.W, 32), (unsigned)ceil_div(s.C, 32), (unsigned)s.B); }
+
+// one fused kernel: its dynamic shared memory, the launch, the launch check
+template <typename... P, typename... A>
+int launch_fused(void (*kern)(P...), const char *name, dim3 grid, int smem, cudaStream_t st, const A &...args) {
+    if (int rc = ensure_dyn_smem((const void *)kern, smem, name)) return rc;
+    kern<<<grid, kDcnThreads, smem, st>>>(args...);
+    return check_launch(name);
+}
+
+// weights WT = float or T; an fp32 bias is used as it is, a T bias through an fp32 copy
 template <typename T, typename WT>
-int dcn_backward_half(const T *input, const WT *weight, const T *offset, int64_t offset_bstride, const T *mask, int64_t mask_bstride,
-                      const T *grad_output, T *grad_input, WT *grad_weight, WT *grad_bias, T *grad_offset, int64_t grad_offset_bstride,
-                      T *grad_mask, int64_t grad_mask_bstride, float scale, unsigned char *ws, int B, int C, int H, int W, int Cout,
-                      int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, cudaStream_t st) {
-    const int Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1, Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
-    const int tiles_x = (int)ceil_div(Wo, 16), tiles_per_sample = tiles_x * (int)ceil_div(Ho, 8), ntiles = B * tiles_per_sample;
-    const int K = kh * kw;
-    const DcnHalfWs L(B, C, H, W, Cout, Ho, Wo, kh, kw);
+int dcn_forward(const DcnShape &s, const T *input, const WT *weight, const WT *bias, const T *offset, int64_t offset_bstride,
+                const T *mask, int64_t mask_bstride, T *output, unsigned char *ws, cudaStream_t st) {
+    typedef DcnElem<T> X;
+    typedef typename X::Mma M;
+    const DcnWs<T> L(s);
+    const int K = s.kh * s.kw;
     T *xh = (T *)ws;
-    float *gxh = (float *)(ws + L.x);
-    T *gt = (T *)(ws + L.x + L.gx);
-    T *wp = (T *)(ws + L.x + L.gx + L.g);
-    float *gw32 = (float *)(ws + L.x + L.gx + L.g + L.w);
+    M *wp[2] = {(M *)(ws + L.x), (M *)(ws + L.x + L.w)};
+    dcn_nchw_to_nhwc_kernel<T><<<transpose_grid(s), 256, 0, st>>>(input, xh, s.C, s.H * s.W);
+    int rc = check_launch("dcn_nchw_to_nhwc_kernel");
+    if (rc) return rc;
+    dcn_weight_pack_kernel<WT, T><<<grid_cap((int64_t)s.Cout * s.C * K, 8), 256, 0, st>>>(weight, s.Cout, s.C, K, wp[0], wp[1]);
+    if ((rc = check_launch("dcn_weight_pack_kernel"))) return rc;
+    DcnFArgsT<T> a;
+    set_shape(a, s);
+    a.ncb = s.C / BK; a.nkb = K * a.ncb;
+    a.xh = xh; a.off = offset; a.msk = mask; a.out = output; a.off_bs = offset_bstride; a.mask_bs = mask_bstride;
+    if constexpr (std::is_same<WT, float>::value) {
+        a.bias = bias;
+    } else if (bias) {
+        float *bf = (float *)(ws + L.fwd_bias());
+        dcn_to_f32_kernel<WT><<<1, 256, 0, st>>>(bias, bf, s.Cout);
+        if ((rc = check_launch("dcn_to_f32_kernel"))) return rc;
+        a.bias = bf;
+    } else {
+        a.bias = nullptr;
+    }
+    CUtensorMap tw[X::kOps];
+    const int64_t Kt = (int64_t)K * s.C;
+    for (int i = 0; i < X::kOps; ++i)
+        if ((rc = make_map(&tw[i], wp[i], Kt, s.Cout, Kt, BK, 128))) return rc;    // 2-byte elements: the bf16 map type only sets the size
+    const int smem = DcnSmem<128, 2, X::kOps>::total(K);     // two stages, not three: the 64 KB saved become L1 for the gathers
+    const dim3 grid((unsigned)s.ntiles, (unsigned)(s.Cout / 128), 1);
+    if constexpr (X::kSplit) return launch_fused(dcn_fwd_tcgen05_kernel<128, 2>, "dcn_fwd_tcgen05_kernel", grid, smem, st, tw[0], tw[1], a);
+    else return launch_fused(dcn_fwd_half_kernel<T>, "dcn_fwd_half_kernel", grid, smem, st, tw[0], a);
+}
+
+// The weight gradient when grad_weight is given, the data gradient when any of grad_input / grad_offset / grad_mask is (weight
+// is read only then); grad_bias is summed here for half precision only (dcn.cu does it for fp32).  grad_weight is accumulated
+// directly when it is fp32, through the fp32 scratch otherwise; grad_input always through the fp32 NHWC scratch.
+template <typename T, typename WT>
+int dcn_backward(const DcnShape &s, const T *input, const WT *weight, const T *offset, int64_t offset_bstride, const T *mask,
+                 int64_t mask_bstride, const T *grad_output, T *grad_input, WT *grad_weight, WT *grad_bias, T *grad_offset,
+                 int64_t grad_offset_bstride, T *grad_mask, int64_t grad_mask_bstride, float scale, unsigned char *ws, cudaStream_t st) {
+    typedef DcnElem<T> X;
+    typedef typename X::Mma M;
+    constexpr bool f32w = std::is_same<WT, float>::value;
+    const DcnWs<T> L(s);
+    const int K = s.kh * s.kw;
+    const int64_t nw = (int64_t)s.Cout * s.C * K;
+    T *xh = (T *)ws;
+    M *gt[2] = {(M *)(ws + L.x), (M *)(ws + L.x + L.g)};
+    M *wp[2] = {(M *)(ws + L.bwd_w()), (M *)(ws + L.bwd_w() + L.w)};
+    float *gxh = (float *)(ws + L.bwd_gx()), *gw32 = (float *)(ws + L.bwd_gw());
     const bool want_data = grad_input || grad_offset || grad_mask;
     int rc = MR_OK;
-    if (grad_bias) {
-        dcn_bias_grad_half_kernel<T, WT><<<Cout, 256, 0, st>>>(grad_output, B, Cout, Ho * Wo, grad_bias);
-        if ((rc = check_launch("dcn_bias_grad_half_kernel"))) return rc;
+    if constexpr (!X::kSplit) {
+        if (grad_bias) {
+            dcn_bias_grad_half_kernel<T, WT><<<s.Cout, 256, 0, st>>>(grad_output, s.B, s.Cout, s.P, grad_bias);
+            if ((rc = check_launch("dcn_bias_grad_half_kernel"))) return rc;
+        }
     }
     if (!want_data && !grad_weight) return MR_OK;
-    if ((rc = dcn_to_nhwc_half(input, xh, B, C, H, W, st))) return rc;
-    const int64_t ng = (int64_t)ntiles * Cout * 8;
-    dcn_go_retile_half_kernel<T><<<grid_cap(ng, 16), 256, 0, st>>>(grad_output, B, Cout, Ho, Wo, tiles_x, tiles_per_sample, gt);
-    if ((rc = check_launch("dcn_go_retile_half_kernel"))) return rc;
+    dcn_nchw_to_nhwc_kernel<T><<<transpose_grid(s), 256, 0, st>>>(input, xh, s.C, s.H * s.W);
+    if ((rc = check_launch("dcn_nchw_to_nhwc_kernel"))) return rc;
+    dcn_go_retile_kernel<T><<<grid_cap((int64_t)s.ntiles * s.Cout * 8, 16), 256, 0, st>>>(grad_output, s.B, s.Cout, s.Ho, s.Wo, s.tiles_x,
+                                                                                          s.tiles_per_sample, gt[0], gt[1]);
+    if ((rc = check_launch("dcn_go_retile_kernel"))) return rc;
     if (grad_weight) {
-        constexpr bool f32w = std::is_same<WT, float>::value;
-        const int64_t nw = (int64_t)Cout * C * K;
         if constexpr (!f32w) MR_CUDA_TRY(cudaMemsetAsync(gw32, 0, (size_t)nw * 4, st), "cudaMemsetAsync(dcn grad_weight scratch)");
         DcnWArgsT<T> a;
-        a.B = B; a.C = C; a.H = H; a.W = W; a.Cout = Cout; a.kh = kh; a.kw = kw; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw; a.dh = dh; a.dw = dw;
-        a.Ho = Ho; a.Wo = Wo; a.P = Ho * Wo; a.tiles_x = tiles_x; a.tiles_per_sample = tiles_per_sample; a.ncb = C / BK; a.nkb = K * a.ncb;
-        a.ntiles = ntiles;
+        set_shape(a, s);
+        a.ncb = s.C / BK; a.nkb = K * a.ncb; a.ntiles = s.ntiles;
         a.xh = xh; a.off = offset; a.msk = mask; a.off_bs = offset_bstride; a.mask_bs = mask_bstride; a.scale = scale;
         a.gw = f32w ? (float *)grad_weight : gw32;
-        CUtensorMap tg;
-        if ((rc = make_map(&tg, gt, BM, (int64_t)ntiles * Cout, BM, BK, BM))) return rc;
-        a.splits = dcn_wgrad_splits(a.nkb, Cout, ntiles);
-        constexpr int smem = DcnWSmemT<1>::TOTAL;
-        { int rc_attr = ensure_dyn_smem((const void *)dcn_wgrad_half_kernel<T>, smem, "dcn_wgrad_half smem attr"); if (rc_attr) return rc_attr; }
-        dim3 grid((unsigned)a.nkb, (unsigned)a.splits, (unsigned)(Cout / BM));
-        dcn_wgrad_half_kernel<T><<<grid, kDcnThreads, smem, st>>>(tg, a);
-        if ((rc = check_launch("dcn_wgrad_half_kernel"))) return rc;
+        a.splits = dcn_wgrad_splits(a.nkb, s.Cout, s.ntiles);
+        CUtensorMap tg[X::kOps];
+        for (int i = 0; i < X::kOps; ++i)
+            if ((rc = make_map(&tg[i], gt[i], BM, (int64_t)s.ntiles * s.Cout, BM, BK, BM))) return rc;
+        const dim3 grid((unsigned)a.nkb, (unsigned)a.splits, (unsigned)(s.Cout / BM));
+        constexpr int smem = DcnWSmemT<X::kOps>::TOTAL;
+        if constexpr (X::kSplit) rc = launch_fused(dcn_wgrad_tcgen05_kernel, "dcn_wgrad_tcgen05_kernel", grid, smem, st, tg[0], tg[1], a);
+        else rc = launch_fused(dcn_wgrad_half_kernel<T>, "dcn_wgrad_half_kernel", grid, smem, st, tg[0], a);
+        if (rc) return rc;
         if constexpr (!f32w) {
             dcn_add_f32_kernel<WT><<<grid_cap(nw, 8), 256, 0, st>>>(gw32, grad_weight, nw);
             if ((rc = check_launch("dcn_add_f32_kernel"))) return rc;
         }
     }
     if (want_data) {
-        if ((rc = dcn_pack_weight_half(weight, wp, Cout, C, K, st))) return rc;
-        if (grad_input) MR_CUDA_TRY(cudaMemsetAsync(gxh, 0, (size_t)B * H * W * C * 4, st), "cudaMemsetAsync(dcn grad_input scratch)");
+        dcn_weight_pack_kernel<WT, T><<<grid_cap(nw, 8), 256, 0, st>>>(weight, s.Cout, s.C, K, wp[0], wp[1]);
+        if ((rc = check_launch("dcn_weight_pack_kernel"))) return rc;
+        if (grad_input) MR_CUDA_TRY(cudaMemsetAsync(gxh, 0, (size_t)s.B * s.H * s.W * s.C * 4, st), "cudaMemsetAsync(dcn grad_input scratch)");
+        typedef DcnDSmemT<X::kOps> D;
         DcnDArgsT<T> a;
-        a.B = B; a.C = C; a.H = H; a.W = W; a.Cout = Cout; a.kh = kh; a.kw = kw; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw; a.dh = dh; a.dw = dw;
-        a.Ho = Ho; a.Wo = Wo; a.P = Ho * Wo; a.tiles_x = tiles_x; a.tiles_per_sample = tiles_per_sample; a.nch = C / 128;
-        a.nkk = Cout / DcnDSmemT<1>::KB;
+        set_shape(a, s);
+        a.nch = s.C / 128; a.nkk = s.Cout / D::KB;
         a.xh = xh; a.off = offset; a.msk = mask; a.gxh = grad_input ? gxh : nullptr; a.goff = grad_offset; a.gmask = grad_mask;
         a.off_bs = offset_bstride; a.mask_bs = mask_bstride; a.goff_bs = grad_offset_bstride; a.gmask_bs = grad_mask_bstride;
-        a.tap_splits = dcn_dgrad_tap_splits(K, ntiles, a.nch);
-        CUtensorMap tg, tw;
-        if ((rc = make_map(&tg, gt, BM, (int64_t)ntiles * Cout, BM, BK, DcnDSmemT<1>::KB))) return rc;
-        if ((rc = make_map(&tw, wp, (int64_t)K * C, Cout, (int64_t)K * C, BK, DcnDSmemT<1>::KB))) return rc;
-        constexpr int smem = DcnDSmemT<1>::TOTAL;
-        { int rc_attr = ensure_dyn_smem((const void *)dcn_dgrad_half_kernel<T>, smem, "dcn_dgrad_half smem attr"); if (rc_attr) return rc_attr; }
-        dim3 grid((unsigned)ntiles, (unsigned)a.tap_splits);
-        dcn_dgrad_half_kernel<T><<<grid, kDcnThreads, smem, st>>>(tg, tw, a);
-        if ((rc = check_launch("dcn_dgrad_half_kernel"))) return rc;
+        a.tap_splits = dcn_dgrad_tap_splits(K, s.ntiles, a.nch);
+        CUtensorMap tg[X::kOps], tw[X::kOps];
+        const int64_t Kt = (int64_t)K * s.C;
+        for (int i = 0; i < X::kOps; ++i) {
+            if ((rc = make_map(&tg[i], gt[i], BM, (int64_t)s.ntiles * s.Cout, BM, BK, D::KB))) return rc;
+            if ((rc = make_map(&tw[i], wp[i], Kt, s.Cout, Kt, BK, D::KB))) return rc;
+        }
+        const dim3 grid((unsigned)s.ntiles, (unsigned)a.tap_splits);
+        if constexpr (X::kSplit) rc = launch_fused(dcn_dgrad_tcgen05_kernel, "dcn_dgrad_tcgen05_kernel", grid, D::TOTAL, st, tg[0], tg[1], tw[0], tw[1], a);
+        else rc = launch_fused(dcn_dgrad_half_kernel<T>, "dcn_dgrad_half_kernel", grid, D::TOTAL, st, tg[0], tw[0], a);
+        if (rc) return rc;
         if (grad_input) {
-            dim3 tgr((unsigned)ceil_div((int64_t)H * W, 32), (unsigned)ceil_div(C, 32), (unsigned)B);
-            dcn_nhwc_to_nchw_add_half_kernel<T><<<tgr, 256, 0, st>>>(gxh, grad_input, C, H * W);
-            if ((rc = check_launch("dcn_nhwc_to_nchw_add_half_kernel"))) return rc;
+            dcn_nhwc_to_nchw_add_kernel<T><<<transpose_grid(s), 256, 0, st>>>(gxh, grad_input, s.C, s.H * s.W);
+            if ((rc = check_launch("dcn_nhwc_to_nchw_add_kernel"))) return rc;
         }
     }
     return MR_OK;
 }
 
-// dtype codes of the C-ABI: 0 = fp32, 1 = bf16, 2 = fp16
+// dtype codes of the C-ABI: 0 = fp32, 1 = bf16, 2 = fp16; half-precision weights are fp32 or the input's type
 enum { kDtF32 = 0, kDtBF16 = 1, kDtF16 = 2 };
-
-// the fused-path conditions shared by the half-precision entry points; MR_OK when the call may go ahead
-int dcn_half_eligible(int dtype, int weight_dtype, int B, int C, int H, int W, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
-                      int dh, int dw, int group, int dg) {
-    if (dtype != kDtBF16 && dtype != kDtF16) return MR_ERR_UNSUPPORTED;
-    if (weight_dtype != kDtF32 && weight_dtype != dtype) return MR_ERR_UNSUPPORTED;
-    if (group != 1 || dg != 1 || C % 64 || Cout % 128 || B <= 0 || H > 65535 || W > 65535) return MR_ERR_UNSUPPORTED;
-    if (getenv("MR_DCN_UNFUSED")) return MR_ERR_UNSUPPORTED;
-    if (kh <= 0 || kw <= 0 || sh <= 0 || sw <= 0 || dh <= 0 || dw <= 0 || ph < 0 || pw < 0 || C <= 0 || H <= 0 || W <= 0) return MR_ERR_BAD_SHAPE;
-    const int Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1, Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
-    if (Ho <= 0 || Wo <= 0) return MR_ERR_BAD_SHAPE;
-    const int64_t ntiles = (int64_t)B * ceil_div(Wo, 16) * ceil_div(Ho, 8);
-    if (ntiles * Cout > 0x7fffffffLL) return MR_ERR_UNSUPPORTED;
-    return MR_OK;
+bool dcn_half_dtypes(int dtype, int weight_dtype) {
+    return (dtype == kDtBF16 || dtype == kDtF16) && (weight_dtype == kDtF32 || weight_dtype == dtype);
 }
 
 }  // namespace
@@ -1327,9 +1291,7 @@ extern "C" {
 
 /* scratch the fused forward needs: NHWC copy of the input + hi/lo packed weights (256-byte aligned pieces) */
 int64_t mr_dcn_fused_workspace_bytes(int64_t B, int64_t C, int64_t H, int64_t W, int64_t Cout, int64_t kh, int64_t kw) {
-    const int64_t x = round_up(B * H * W * C * 4, 256);
-    const int64_t w = round_up(Cout * C * kh * kw * 2, 256);
-    return x + 2 * w;
+    return DcnWs<float>(B, C, H, W, Cout, 1, 1, kh, kw).forward();
 }
 
 /* MR_ERR_UNSUPPORTED when the shape is outside the fused path (the caller then runs the unfused kernels of dcn.cu). */
@@ -1337,54 +1299,19 @@ int mr_dcn_forward_fused_f32(const float *input, const float *weight, const floa
                              int64_t offset_bstride, const float *mask, int64_t mask_bstride, float *output,
                              float *workspace, int64_t workspace_bytes, int B, int C, int H, int W, int Cout, int kh, int kw,
                              int sh, int sw, int ph, int pw, int dh, int dw, int group, int dg, void *stream) {
-    if (group != 1 || dg != 1 || C % 64 || Cout % 128 || B <= 0 || H > 65535 || W > 65535) return MR_ERR_UNSUPPORTED;
-    if (getenv("MR_DCN_UNFUSED")) return MR_ERR_UNSUPPORTED;
+    DcnShape s;
+    int rc = dcn_shape<float>(s, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg, kFwd);
+    if (rc) return rc;
     if (!input || !weight || !offset || !output || !workspace) return MR_ERR_NULL_POINTER;
     if (workspace_bytes < mr_dcn_fused_workspace_bytes(B, C, H, W, Cout, kh, kw) || ((uintptr_t)workspace % 256)) return MR_ERR_UNSUPPORTED;
-    DcnFArgs a;
-    a.B = B; a.C = C; a.H = H; a.W = W; a.Cout = Cout; a.kh = kh; a.kw = kw; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw;
-    a.dh = dh; a.dw = dw;
-    a.Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1;
-    a.Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
-    if (a.Ho <= 0 || a.Wo <= 0) return MR_ERR_BAD_SHAPE;
-    a.P = a.Ho * a.Wo;
-    a.tiles_x = (int)ceil_div(a.Wo, 16);
-    a.tiles_per_sample = a.tiles_x * (int)ceil_div(a.Ho, 8);
-    a.ncb = C / BK; a.nkb = kh * kw * a.ncb;
-    if ((int64_t)B * a.tiles_per_sample > 0x7fffffffLL) return MR_ERR_UNSUPPORTED;
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned char *ws = (unsigned char *)workspace;
-    float *xh = (float *)ws;
-    const int64_t xbytes = round_up((int64_t)B * H * W * C * 4, 256), wbytes = round_up((int64_t)Cout * C * kh * kw * 2, 256);
-    bf16 *whi = (bf16 *)(ws + xbytes), *wlo = (bf16 *)(ws + xbytes + wbytes);
-    {
-        dim3 tg((unsigned)ceil_div((int64_t)H * W, 32), (unsigned)ceil_div(C, 32), (unsigned)B);
-        dcn_nchw_to_nhwc_kernel<<<tg, 256, 0, st>>>(input, xh, C, H * W);
-    }
-    int rc = check_launch("dcn_nchw_to_nhwc_kernel");
-    if (rc) return rc;
-    const int64_t nw = (int64_t)Cout * C * kh * kw;
-    dcn_weight_pack_kernel<<<(unsigned)std::min<int64_t>(ceil_div(nw, 256), sm_count() * 8), 256, 0, st>>>(weight, Cout, C, kh * kw, whi, wlo);
-    rc = check_launch("dcn_weight_pack_kernel");
-    if (rc) return rc;
-    a.xh = xh; a.off = offset; a.msk = mask; a.bias = bias; a.out = output; a.off_bs = offset_bstride; a.mask_bs = mask_bstride;
-    const int64_t Kt = (int64_t)kh * kw * C;
-    CUtensorMap th, tl;
-    rc = make_map(&th, whi, Kt, Cout, Kt, BK, 128);
-    if (rc) return rc;
-    rc = make_map(&tl, wlo, Kt, Cout, Kt, BK, 128);
-    if (rc) return rc;
-    /* two stages, not three: the 64 KB saved become L1 for the gathers (MR_DCN_STAGES3 selects three for experiments) */
-    const bool three = getenv("MR_DCN_STAGES3") != nullptr;
-    if (three) return launch_dcn_fwd<128, 3>(th, tl, a, st);
-    return launch_dcn_fwd<128, 2>(th, tl, a, st);
+    return dcn_forward<float, float>(s, input, weight, bias, offset, offset_bstride, mask, mask_bstride, output,
+                                     (unsigned char *)workspace, (cudaStream_t)stream);
 }
 
 /* scratch of the fused backward: NHWC copies of the input and of grad_input, re-tiled hi / lo grad_output, packed hi / lo weights */
 int64_t mr_dcn_fused_backward_workspace_bytes(int64_t B, int64_t C, int64_t H, int64_t W, int64_t Cout, int64_t Ho, int64_t Wo,
                                               int64_t kh, int64_t kw) {
-    const int64_t tiles = ceil_div(Wo, 16) * ceil_div(Ho, 8);
-    return 2 * round_up(B * H * W * C * 4, 256) + 2 * round_up(B * tiles * Cout * BM * 2, 256) + 2 * round_up(Cout * C * kh * kw * 2, 256);
+    return DcnWs<float>(B, C, H, W, Cout, Ho, Wo, kh, kw).backward();
 }
 
 /* The whole of mr_dcn_backward_f32 except grad_bias on the fused kernels (weight gradient + data gradient); MR_ERR_UNSUPPORTED
@@ -1394,82 +1321,20 @@ int mr_dcn_backward_fused_f32(const float *input, const float *weight, const flo
                               float *grad_offset, int64_t grad_offset_bstride, float *grad_mask, int64_t grad_mask_bstride,
                               float weight_grad_scale, float *workspace, int64_t workspace_bytes, int B, int C, int H, int W, int Cout,
                               int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int group, int dg, void *stream) {
-    if (group != 1 || dg != 1 || C % 128 || Cout % 128 || B <= 0 || H > 65535 || W > 65535) return MR_ERR_UNSUPPORTED;
-    if (getenv("MR_DCN_UNFUSED") || getenv("MR_DCN_UNFUSED_DGRAD")) return MR_ERR_UNSUPPORTED;
+    DcnShape s;
+    // all or nothing: the data-gradient conditions hold whatever the call wants (mr_dcn_wgrad_fused_f32 is the partial entry)
+    int rc = dcn_shape<float>(s, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg, kDgrad);
+    if (rc) return rc;
     if (!input || !weight || !offset || !grad_output || !workspace) return MR_ERR_NULL_POINTER;
-    const int Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1, Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
-    if (Ho <= 0 || Wo <= 0) return MR_ERR_BAD_SHAPE;
-    if (workspace_bytes < mr_dcn_fused_backward_workspace_bytes(B, C, H, W, Cout, Ho, Wo, kh, kw) || ((uintptr_t)workspace % 256)) return MR_ERR_UNSUPPORTED;
-    const int tiles_x = (int)ceil_div(Wo, 16), tiles_per_sample = tiles_x * (int)ceil_div(Ho, 8), ntiles = B * tiles_per_sample;
-    if ((int64_t)ntiles * Cout > 0x7fffffffLL) return MR_ERR_UNSUPPORTED;
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned char *ws = (unsigned char *)workspace;
-    const int64_t xbytes = round_up((int64_t)B * H * W * C * 4, 256), gbytes = round_up((int64_t)ntiles * Cout * BM * 2, 256);
-    const int64_t wbytes = round_up((int64_t)Cout * C * kh * kw * 2, 256);
-    float *xh = (float *)ws, *gxh = (float *)(ws + xbytes);
-    bf16 *ghi = (bf16 *)(ws + 2 * xbytes), *glo = (bf16 *)(ws + 2 * xbytes + gbytes);
-    bf16 *whi = (bf16 *)(ws + 2 * xbytes + 2 * gbytes), *wlo = (bf16 *)(ws + 2 * xbytes + 2 * gbytes + wbytes);
-    const bool want_data = grad_input || grad_offset || grad_mask;
-    if (!want_data && !grad_weight) return MR_OK;
-    {
-        dim3 tg((unsigned)ceil_div((int64_t)H * W, 32), (unsigned)ceil_div(C, 32), (unsigned)B);
-        dcn_nchw_to_nhwc_kernel<<<tg, 256, 0, st>>>(input, xh, C, H * W);
-    }
-    int rc = check_launch("dcn_nchw_to_nhwc_kernel");
-    if (rc) return rc;
-    const int64_t ng = (int64_t)ntiles * Cout * 8;
-    dcn_go_retile_kernel<<<(unsigned)std::min<int64_t>(ceil_div(ng, 256), (int64_t)sm_count() * 16), 256, 0, st>>>(
-        grad_output, B, Cout, Ho, Wo, tiles_x, tiles_per_sample, ghi, glo);
-    rc = check_launch("dcn_go_retile_kernel");
-    if (rc) return rc;
-    if (grad_weight) {
-        DcnWArgs a;
-        a.B = B; a.C = C; a.H = H; a.W = W; a.Cout = Cout; a.kh = kh; a.kw = kw; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw; a.dh = dh; a.dw = dw;
-        a.Ho = Ho; a.Wo = Wo; a.P = Ho * Wo; a.tiles_x = tiles_x; a.tiles_per_sample = tiles_per_sample; a.ncb = C / BK; a.nkb = kh * kw * a.ncb;
-        a.ntiles = ntiles;
-        a.xh = xh; a.off = offset; a.msk = mask; a.off_bs = offset_bstride; a.mask_bs = mask_bstride; a.gw = grad_weight; a.scale = weight_grad_scale;
-        rc = launch_dcn_wgrad(a, ghi, glo, st);
-        if (rc) return rc;
-    }
-    if (want_data) {
-        const int64_t nw = (int64_t)Cout * C * kh * kw;
-        dcn_weight_pack_kernel<<<(unsigned)std::min<int64_t>(ceil_div(nw, 256), sm_count() * 8), 256, 0, st>>>(weight, Cout, C, kh * kw, whi, wlo);
-        rc = check_launch("dcn_weight_pack_kernel");
-        if (rc) return rc;
-        if (grad_input) MR_CUDA_TRY(cudaMemsetAsync(gxh, 0, (size_t)B * H * W * C * 4, st), "cudaMemsetAsync(dcn grad_input scratch)");
-        DcnDArgs a;
-        a.B = B; a.C = C; a.H = H; a.W = W; a.Cout = Cout; a.kh = kh; a.kw = kw; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw; a.dh = dh; a.dw = dw;
-        a.Ho = Ho; a.Wo = Wo; a.P = Ho * Wo; a.tiles_x = tiles_x; a.tiles_per_sample = tiles_per_sample; a.nch = C / 128; a.nkk = Cout / DcnDSmem::KB;
-        a.xh = xh; a.off = offset; a.msk = mask; a.gxh = grad_input ? gxh : nullptr; a.goff = grad_offset; a.gmask = grad_mask;
-        a.off_bs = offset_bstride; a.mask_bs = mask_bstride; a.goff_bs = grad_offset_bstride; a.gmask_bs = grad_mask_bstride;
-        const int K = kh * kw;
-        const int splits = dcn_dgrad_tap_splits(K, ntiles, a.nch);
-        a.tap_splits = splits;
-        CUtensorMap gh, gl, wh, wl;
-        const int64_t Kt = (int64_t)K * C;
-        if ((rc = make_map(&gh, ghi, BM, (int64_t)ntiles * Cout, BM, BK, DcnDSmem::KB))) return rc;
-        if ((rc = make_map(&gl, glo, BM, (int64_t)ntiles * Cout, BM, BK, DcnDSmem::KB))) return rc;
-        if ((rc = make_map(&wh, whi, Kt, Cout, Kt, BK, DcnDSmem::KB))) return rc;
-        if ((rc = make_map(&wl, wlo, Kt, Cout, Kt, BK, DcnDSmem::KB))) return rc;
-        { int rc_attr = ensure_dyn_smem((const void *)dcn_dgrad_tcgen05_kernel, DcnDSmem::TOTAL, "dcn_dgrad_tcgen05 smem attr"); if (rc_attr) return rc_attr; }
-        dim3 grid((unsigned)ntiles, (unsigned)splits);
-        dcn_dgrad_tcgen05_kernel<<<grid, kDcnThreads, DcnDSmem::TOTAL, st>>>(gh, gl, wh, wl, a);
-        rc = check_launch("dcn_dgrad_tcgen05_kernel");
-        if (rc) return rc;
-        if (grad_input) {
-            dim3 tg((unsigned)ceil_div((int64_t)H * W, 32), (unsigned)ceil_div(C, 32), (unsigned)B);
-            dcn_nhwc_to_nchw_add_kernel<<<tg, 256, 0, st>>>(gxh, grad_input, C, H * W);
-            rc = check_launch("dcn_nhwc_to_nchw_add_kernel");
-            if (rc) return rc;
-        }
-    }
-    return MR_OK;
+    if (workspace_bytes < mr_dcn_fused_backward_workspace_bytes(B, C, H, W, Cout, s.Ho, s.Wo, kh, kw) || ((uintptr_t)workspace % 256)) return MR_ERR_UNSUPPORTED;
+    return dcn_backward<float, float>(s, input, weight, offset, offset_bstride, mask, mask_bstride, grad_output, grad_input, grad_weight,
+                                      nullptr, grad_offset, grad_offset_bstride, grad_mask, grad_mask_bstride, weight_grad_scale,
+                                      (unsigned char *)workspace, (cudaStream_t)stream);
 }
 
 /* scratch of the fused weight gradient: NHWC copy of the input + re-tiled hi / lo grad_output */
 int64_t mr_dcn_fused_wgrad_workspace_bytes(int64_t B, int64_t C, int64_t H, int64_t W, int64_t Cout, int64_t Ho, int64_t Wo) {
-    const int64_t tiles = ceil_div(Wo, 16) * ceil_div(Ho, 8);
-    return round_up(B * H * W * C * 4, 256) + 2 * round_up(B * tiles * Cout * BM * 2, 256);
+    return DcnWs<float>(B, C, H, W, Cout, Ho, Wo, 1, 1).wgrad();
 }
 
 /* grad_weight [Cout][C][kh*kw] += scale * (grad_output (*) deformable columns); MR_ERR_UNSUPPORTED outside the fused path. */
@@ -1477,53 +1342,27 @@ int mr_dcn_wgrad_fused_f32(const float *input, const float *offset, int64_t offs
                            const float *grad_output, float *grad_weight, float scale, float *workspace, int64_t workspace_bytes,
                            int B, int C, int H, int W, int Cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw,
                            int group, int dg, void *stream) {
-    if (group != 1 || dg != 1 || C % 64 || Cout % 128 || B <= 0 || H > 65535 || W > 65535) return MR_ERR_UNSUPPORTED;
-    if (getenv("MR_DCN_UNFUSED") || getenv("MR_DCN_UNFUSED_WGRAD")) return MR_ERR_UNSUPPORTED;
+    DcnShape s;
+    int rc = dcn_shape<float>(s, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg, kWgrad);
+    if (rc) return rc;
     if (!input || !offset || !grad_output || !grad_weight || !workspace) return MR_ERR_NULL_POINTER;
-    DcnWArgs a;
-    a.B = B; a.C = C; a.H = H; a.W = W; a.Cout = Cout; a.kh = kh; a.kw = kw; a.sh = sh; a.sw = sw; a.ph = ph; a.pw = pw;
-    a.dh = dh; a.dw = dw;
-    a.Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1;
-    a.Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
-    if (a.Ho <= 0 || a.Wo <= 0) return MR_ERR_BAD_SHAPE;
-    if (workspace_bytes < mr_dcn_fused_wgrad_workspace_bytes(B, C, H, W, Cout, a.Ho, a.Wo) || ((uintptr_t)workspace % 256)) return MR_ERR_UNSUPPORTED;
-    a.P = a.Ho * a.Wo;
-    a.tiles_x = (int)ceil_div(a.Wo, 16);
-    a.tiles_per_sample = a.tiles_x * (int)ceil_div(a.Ho, 8);
-    a.ncb = C / BK; a.nkb = kh * kw * a.ncb;
-    a.ntiles = B * a.tiles_per_sample;
-    if ((int64_t)a.ntiles * Cout > 0x7fffffffLL) return MR_ERR_UNSUPPORTED;
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned char *ws = (unsigned char *)workspace;
-    float *xh = (float *)ws;
-    const int64_t xbytes = round_up((int64_t)B * H * W * C * 4, 256), gbytes = round_up((int64_t)a.ntiles * Cout * BM * 2, 256);
-    bf16 *ghi = (bf16 *)(ws + xbytes), *glo = (bf16 *)(ws + xbytes + gbytes);
-    {
-        dim3 tg((unsigned)ceil_div((int64_t)H * W, 32), (unsigned)ceil_div(C, 32), (unsigned)B);
-        dcn_nchw_to_nhwc_kernel<<<tg, 256, 0, st>>>(input, xh, C, H * W);
-    }
-    int rc = check_launch("dcn_nchw_to_nhwc_kernel");
-    if (rc) return rc;
-    const int64_t ng = (int64_t)a.ntiles * Cout * 8;
-    dcn_go_retile_kernel<<<(unsigned)std::min<int64_t>(ceil_div(ng, 256), (int64_t)sm_count() * 16), 256, 0, st>>>(
-        grad_output, B, Cout, a.Ho, a.Wo, a.tiles_x, a.tiles_per_sample, ghi, glo);
-    rc = check_launch("dcn_go_retile_kernel");
-    if (rc) return rc;
-    a.xh = xh; a.off = offset; a.msk = mask; a.off_bs = offset_bstride; a.mask_bs = mask_bstride; a.gw = grad_weight; a.scale = scale;
-    return launch_dcn_wgrad(a, ghi, glo, st);
+    if (workspace_bytes < mr_dcn_fused_wgrad_workspace_bytes(B, C, H, W, Cout, s.Ho, s.Wo) || ((uintptr_t)workspace % 256)) return MR_ERR_UNSUPPORTED;
+    return dcn_backward<float, float>(s, input, nullptr, offset, offset_bstride, mask, mask_bstride, grad_output, nullptr, grad_weight,
+                                      nullptr, nullptr, 0, nullptr, 0, scale, (unsigned char *)workspace, (cudaStream_t)stream);
 }
 
 /* ---- half precision: dtype 1 = bf16, 2 = fp16 for input / offset / mask / output / grad_output / grad_input / grad_offset /
  * grad_mask; weight_dtype 0 = fp32 or the same code as dtype for weight / bias / grad_weight / grad_bias. */
 int64_t mr_dcn_fused_workspace_bytes_h(int64_t B, int64_t C, int64_t H, int64_t W, int64_t Cout, int64_t kh, int64_t kw) {
-    return DcnHalfWs(B, C, H, W, Cout, 1, 1, kh, kw).forward();
+    return DcnWs<__half>(B, C, H, W, Cout, 1, 1, kh, kw).forward();
 }
 
 int64_t mr_dcn_fused_backward_workspace_bytes_h(int64_t B, int64_t C, int64_t H, int64_t W, int64_t Cout, int64_t Ho, int64_t Wo,
                                                 int64_t kh, int64_t kw) {
-    return DcnHalfWs(B, C, H, W, Cout, Ho, Wo, kh, kw).backward();
+    return DcnWs<__half>(B, C, H, W, Cout, Ho, Wo, kh, kw).backward();
 }
 
+// (__half stands for both half types in dcn_shape and DcnWs: they have the same operand count and element size)
 #define MR_DCN_HALF_DISPATCH(CALL)                                                                                       \
     if (dtype == kDtBF16 && weight_dtype == kDtF32) { typedef bf16 T; typedef float WT; return CALL; }                   \
     if (dtype == kDtBF16) { typedef bf16 T; typedef bf16 WT; return CALL; }                                              \
@@ -1534,13 +1373,14 @@ int mr_dcn_forward_fused_h(const void *input, const void *weight, const void *bi
                            const void *mask, int64_t mask_bstride, void *output, void *workspace, int64_t workspace_bytes, int B,
                            int C, int H, int W, int Cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int group,
                            int dg, int dtype, int weight_dtype, void *stream) {
-    int rc = dcn_half_eligible(dtype, weight_dtype, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg);
+    if (!dcn_half_dtypes(dtype, weight_dtype)) return MR_ERR_UNSUPPORTED;
+    DcnShape s;
+    int rc = dcn_shape<__half>(s, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg, kFwd);
     if (rc) return rc;
     if (!input || !weight || !offset || !output || !workspace) return MR_ERR_NULL_POINTER;
     if (workspace_bytes < mr_dcn_fused_workspace_bytes_h(B, C, H, W, Cout, kh, kw) || ((uintptr_t)workspace % 256)) return MR_ERR_UNSUPPORTED;
-    MR_DCN_HALF_DISPATCH((dcn_forward_half<T, WT>((const T *)input, (const WT *)weight, (const WT *)bias, (const T *)offset, offset_bstride,
-                                                  (const T *)mask, mask_bstride, (T *)output, (unsigned char *)workspace, B, C, H, W, Cout,
-                                                  kh, kw, sh, sw, ph, pw, dh, dw, (cudaStream_t)stream)))
+    MR_DCN_HALF_DISPATCH((dcn_forward<T, WT>(s, (const T *)input, (const WT *)weight, (const WT *)bias, (const T *)offset, offset_bstride,
+                                             (const T *)mask, mask_bstride, (T *)output, (unsigned char *)workspace, (cudaStream_t)stream)))
 }
 
 /* grad_input / grad_weight / grad_bias accumulate, grad_offset / grad_mask are assigned, as in mr_dcn_backward_f32.  The data
@@ -1551,20 +1391,18 @@ int mr_dcn_backward_fused_h(const void *input, const void *weight, const void *o
                             float weight_grad_scale, void *workspace, int64_t workspace_bytes, int B, int C, int H, int W, int Cout,
                             int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int group, int dg, int dtype,
                             int weight_dtype, void *stream) {
-    int rc = dcn_half_eligible(dtype, weight_dtype, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg);
+    if (!dcn_half_dtypes(dtype, weight_dtype)) return MR_ERR_UNSUPPORTED;
+    const int parts = (grad_weight ? kWgrad : 0) | (grad_input || grad_offset || grad_mask ? kDgrad : 0);
+    DcnShape s;
+    int rc = dcn_shape<__half>(s, B, C, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, group, dg, parts);
     if (rc) return rc;
-    const bool want_data = grad_input || grad_offset || grad_mask;
-    if (want_data && (C % 128 || getenv("MR_DCN_UNFUSED_DGRAD"))) return MR_ERR_UNSUPPORTED;
-    if (grad_weight && getenv("MR_DCN_UNFUSED_WGRAD")) return MR_ERR_UNSUPPORTED;
     if (!input || !weight || !offset || !grad_output || !workspace) return MR_ERR_NULL_POINTER;
-    const int Ho = (H + 2 * ph - (dh * (kh - 1) + 1)) / sh + 1, Wo = (W + 2 * pw - (dw * (kw - 1) + 1)) / sw + 1;
-    if (workspace_bytes < mr_dcn_fused_backward_workspace_bytes_h(B, C, H, W, Cout, Ho, Wo, kh, kw) || ((uintptr_t)workspace % 256))
+    if (workspace_bytes < mr_dcn_fused_backward_workspace_bytes_h(B, C, H, W, Cout, s.Ho, s.Wo, kh, kw) || ((uintptr_t)workspace % 256))
         return MR_ERR_UNSUPPORTED;
-    MR_DCN_HALF_DISPATCH((dcn_backward_half<T, WT>((const T *)input, (const WT *)weight, (const T *)offset, offset_bstride, (const T *)mask,
-                                                   mask_bstride, (const T *)grad_output, (T *)grad_input, (WT *)grad_weight, (WT *)grad_bias,
-                                                   (T *)grad_offset, grad_offset_bstride, (T *)grad_mask, grad_mask_bstride,
-                                                   weight_grad_scale, (unsigned char *)workspace, B, C, H, W, Cout, kh, kw, sh, sw, ph,
-                                                   pw, dh, dw, (cudaStream_t)stream)))
+    MR_DCN_HALF_DISPATCH((dcn_backward<T, WT>(s, (const T *)input, (const WT *)weight, (const T *)offset, offset_bstride, (const T *)mask,
+                                              mask_bstride, (const T *)grad_output, (T *)grad_input, (WT *)grad_weight, (WT *)grad_bias,
+                                              (T *)grad_offset, grad_offset_bstride, (T *)grad_mask, grad_mask_bstride,
+                                              weight_grad_scale, (unsigned char *)workspace, (cudaStream_t)stream)))
 }
 #undef MR_DCN_HALF_DISPATCH
 

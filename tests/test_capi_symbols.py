@@ -69,6 +69,28 @@ def test_argument_validation_without_gpu(so_path):
     assert gemm(0, 1, None, 0, 0.5, 1) == _lib.MR_ERR_UNSUPPORTED
 
 
+def test_dcn_fused_workspace_sizes(so_path):
+    """The five fused-DCN workspace sizes against their closed forms: r() rounds a piece up to 256 bytes; the pieces are the
+    NHWC input copy, the fp32 NHWC grad_input scratch, the re-tiled grad_output and the packed weights (bf16 hi and lo for
+    fp32, one copy for half precision), and for half precision the fp32 bias copy and grad_weight scratch."""
+    import itertools
+    from megreader_b200 import _lib
+    L = _lib.lib()
+    r = lambda n: -(-n // 256) * 256  # noqa: E731
+    shapes = itertools.product((1, 3, 8), (64, 127, 256, 512), ((7, 9), (33, 65), (64, 64)), (128, 384), (1, 3, 5),
+                               ((1, 1), (7, 15), (9, 17), (32, 64), (33, 65)))
+    for B, C, (H, W), Cout, k, (Ho, Wo) in shapes:
+        K, tiles = k * k, -(-Wo // 16) * -(-Ho // 8)
+        x4, g, w = r(4 * B * H * W * C), r(256 * B * tiles * Cout), r(2 * Cout * C * K)
+        shape = (B, C, H, W, Cout, k, k, Ho, Wo)
+        assert L.mr_dcn_fused_workspace_bytes(B, C, H, W, Cout, k, k) == x4 + 2 * w, shape
+        assert L.mr_dcn_fused_wgrad_workspace_bytes(B, C, H, W, Cout, Ho, Wo) == x4 + 2 * g, shape
+        assert L.mr_dcn_fused_backward_workspace_bytes(B, C, H, W, Cout, Ho, Wo, k, k) == 2 * x4 + 2 * g + 2 * w, shape
+        assert L.mr_dcn_fused_workspace_bytes_h(B, C, H, W, Cout, k, k) == r(2 * B * H * W * C) + w + r(4 * Cout), shape
+        assert (L.mr_dcn_fused_backward_workspace_bytes_h(B, C, H, W, Cout, Ho, Wo, k, k)
+                == r(2 * B * H * W * C) + x4 + g + w + r(4 * Cout * C * K)), shape
+
+
 def test_product_never_imports_oracle():
     for path in glob.glob(os.path.join(ROOT, "megreader_b200", "**", "*.py"), recursive=True):
         src = open(path).read()

@@ -74,16 +74,45 @@ def test_dcn_forward_backward_vs_oracle(cuda, case):
 FUSED_FWD_CASE = 8      # stride 2, ragged tiles: the fused wgmma forward
 
 
-@pytest.mark.parametrize("stages3", [False, True], ids=["2stages", "3stages"])
-def test_dcn_fused_forward_rings(cuda, stages3, monkeypatch):
-    """the fused forward with its default two-stage ring and with MR_DCN_STAGES3=1 (read on every call)."""
-    monkeypatch.delenv("MR_DCN_STAGES3", raising=False)
-    if stages3:
-        monkeypatch.setenv("MR_DCN_STAGES3", "1")
+def test_dcn_fused_forward_rings(cuda):
+    """the fused forward runs its one instantiation (the two-stage ring)."""
     wv.run_variant(wv.expected_variant("dcn_fwd"), lambda: test_dcn_forward_backward_vs_oracle(cuda, CASES[FUSED_FWD_CASE]))
 
 
-VARIANTS = {wv.expected_variant("dcn_fwd", env={}), wv.expected_variant("dcn_fwd", env={"MR_DCN_STAGES3": "1"})}
+VARIANTS = {wv.expected_variant("dcn_fwd")}
+
+
+@pytest.mark.parametrize("dt", [torch.float32, torch.float16, torch.bfloat16], ids=["fp32", "fp16", "bf16"])
+def test_dcn_fused_backward_unaligned_grad_output(cuda, dt):
+    """grad_output a contiguous view one element into a larger buffer, so not 16-byte aligned: the fused backward gives the
+    gradients of an aligned copy, bit for bit.  Wo = 16 is one whole tile row, so the aligned call re-tiles grad_output with
+    16-byte loads.  A 3 x 3 kernel at stride 3 with zero offsets samples every input pixel once, and B = 1 with Ho = 8 is one
+    pixel tile (one weight-gradient split), so every atomic sum has one term and the gradients are deterministic."""
+    from megreader_b200 import dcn
+    B, C, H, W, Cout, k, s = 1, 128, 24, 48, 128, 3, 3
+    Ho, Wo = H // s, W // s
+    gen = torch.Generator().manual_seed(11)
+    rnd = lambda *shape, scale=1.0: (torch.randn(*shape, generator=gen) * scale).to(cuda, dt)  # noqa: E731
+    x, w, b = rnd(B, C, H, W), rnd(Cout, C, k, k, scale=(C * k * k) ** -0.5), rnd(Cout)
+    off = torch.zeros(B, 2 * k * k, Ho, Wo, device=cuda, dtype=dt)
+    m = torch.sigmoid(rnd(B, k * k, Ho, Wo))
+    go = rnd(B, Cout, Ho, Wo)
+    buf = torch.empty(go.numel() + 1, device=cuda, dtype=dt)
+    go_view = buf[1:].view(go.shape)
+    go_view.copy_(go)
+    assert go_view.is_contiguous() and go_view.data_ptr() % 16 != 0 and go.data_ptr() % 16 == 0
+
+    def grads(grad_output):
+        g = [torch.zeros_like(t) for t in (x, w, b, off, m)]
+        dcn.modulated_deform_conv_cuda_backward(x, w, b, None, off, m, None, *g, grad_output, k, k, s, s, 0, 0, 1, 1, 1, 1,
+                                                True)
+        torch.cuda.synchronize()
+        return g
+
+    want, got = grads(go), grads(go_view)
+    for name, a, e in zip(("grad_input", "grad_weight", "grad_bias", "grad_offset", "grad_mask"), got, want):
+        assert e.abs().sum() > 0, name
+        assert torch.equal(a, e), name
 
 
 def test_dcn_stride2_offset_slice_quirk(cuda):

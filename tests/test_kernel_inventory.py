@@ -33,7 +33,7 @@ def compiled_variants(so_path):
                     reason="needs cuobjdump and cu++filt from the CUDA toolkit")
 def test_compiled_instantiations_are_the_known_variants(so_path):
     found = compiled_variants(so_path)
-    assert len(wv.ALL_VARIANTS) == 20
+    assert len(wv.ALL_VARIANTS) == 19
     assert found == wv.ALL_VARIANTS, ("not in ALL_VARIANTS: %s; not compiled: %s"
                                       % (sorted(found - wv.ALL_VARIANTS), sorted(wv.ALL_VARIANTS - found)))
 

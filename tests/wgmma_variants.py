@@ -25,7 +25,7 @@ ALL_VARIANTS = frozenset([
     "conv_wgrad_tcgen05_kernel<128,64,6>", "conv_wgrad_tcgen05_kernel<128,80,4>",
     "conv_wgrad_tcgen05_kernel<64,64,8>", "conv_wgrad_tcgen05_kernel<64,80,6>",
     "lstm_step_fwd_tcgen05_kernel<4>", "lstm_step_bwd_tcgen05_kernel<6>",
-    "dcn_fwd_tcgen05_kernel<128,2>", "dcn_fwd_tcgen05_kernel<128,3>",
+    "dcn_fwd_tcgen05_kernel<128,2>",
 ])
 
 _TEMPLATE = re.compile(r"(\w+_kernel)<([^<>]*)>")
@@ -122,9 +122,8 @@ def conv_wgrad_variant(H, W, C, kh, kw, sh=1, sw=1, ph=0, pw=0, dh=1, dw=1, **_)
     return "conv_wgrad_tcgen05_kernel<%d,%d,%d>" % (bn, rb, stages)
 
 
-def dcn_fwd_variant(env=None, **_):
-    env = os.environ if env is None else env
-    return "dcn_fwd_tcgen05_kernel<128,%d>" % (3 if "MR_DCN_STAGES3" in env else 2)
+def dcn_fwd_variant(**_):
+    return "dcn_fwd_tcgen05_kernel<128,2>"
 
 
 _DISPATCH = {
