@@ -86,8 +86,9 @@ template <typename T> struct DcnFArgsT {
 };
 
 // OPS = 2: fp32 input (hi and lo of both operands), 1: half precision
-template <int BN, int STAGES, int OPS = 2>
+template <int BN, int STAGES_, int OPS = 2>
 struct DcnSmem {
+    static constexpr int STAGES = STAGES_;
     static constexpr int A_BYTES = BM * BK * 2;               // one of (hi, lo)
     static constexpr int B_BYTES = BN * BK * 2;
     static constexpr int STAGE_BYTES = OPS * A_BYTES + OPS * B_BYTES;
@@ -103,23 +104,12 @@ constexpr int kProducerThreads = 512;      // 16 warps x (4 rows x 8 channel lan
 constexpr int kDcnMma0 = 640;                 // producer warps end at 576; padded to a warpgroup boundary
 constexpr int kDcnThreads = kDcnMma0 + kMmaThreads;
 
-__device__ __forceinline__ void mbar_arrive_cta(uint64_t *bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
 // The forward body.  T = float: operands hi / lo from tmWh / tmWl, three MMAs per K block; T = __half / bf16: one operand
 // (tmWl is not read), one MMA per K block.
 template <typename T, int BN, int STAGES>
 __device__ __forceinline__ void dcn_fwd_body(const CUtensorMap &tmWh, const CUtensorMap &tmWl, const DcnFArgsT<T> &a) {
     typedef DcnElem<T> X;
     using L = DcnSmem<BN, STAGES, X::kOps>;
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
-    uint64_t *empty = full + STAGES;
-    uint64_t *tmem_full = empty + STAGES;
-    float4 *tapw = (float4 *)(smem + L::TAP_OFF);             // [taps][128] bilinear weights
-    uint2 *tapc = (uint2 *)(tapw + BM * a.kh * a.kw);         // [taps][128] clamped corner rows / columns
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int b = blockIdx.x / a.tiles_per_sample;
     const int tile = blockIdx.x - b * a.tiles_per_sample;
@@ -128,15 +118,15 @@ __device__ __forceinline__ void dcn_fwd_body(const CUtensorMap &tmWh, const CUte
     const int ty0 = (tile / a.tiles_x) * 8, tx0 = (tile % a.tiles_x) * 16;
     const int n0 = blockIdx.y * BN;
     const int nkb = a.nkb;
-
-    if (warp == 0 && lane == 0) {
+    const int tap_rows = BM * a.kh * a.kw;
+    const Ring rg = ring_init<L>(warp == 0 && lane == 0, 1 + kProducerThreads, [&] {
         tma_prefetch_desc(&tmWh);
         if constexpr (X::kSplit) tma_prefetch_desc(&tmWl);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1 + kProducerThreads); mbar_init(empty + s, 1); }
-        mbar_init(tmem_full, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
+    });
+    unsigned char *smem = rg.smem;
+    uint64_t *full = rg.full, *empty = rg.empty, *acc_full = rg.acc_full;
+    float4 *tapw = (float4 *)(smem + L::TAP_OFF);             // [taps][128] bilinear weights
+    uint2 *tapc = (uint2 *)(tapw + tap_rows);                 // [taps][128] clamped corner rows / columns
     float *acc_tile = (float *)smem;                         // laid over the drained operand ring when the K loop is over
     static_assert(L::BAR_OFF >= AccTile<BN>::BYTES, "the accumulator tile must end before the barriers");
 
@@ -148,35 +138,22 @@ __device__ __forceinline__ void dcn_fwd_body(const CUtensorMap &tmWh, const CUte
         constexpr int PASSES = X::kSplit ? 3 : 1;
         const int mt = threadIdx.x - kDcnMma0;
         AccTile<BN> acc;
-        uint64_t *pending = nullptr;
-        for (int i = 0; i < nkb; ++i) {
-            const int s = i % STAGES;
-            mbar_wait(full + s, (i / STAGES) & 1);
+        mma_ring(nkb, STAGES, full, empty, mt == 0, [&](int i, int s) {
             const uint32_t ah = smem_u32(smem + s * L::STAGE_BYTES);
             const uint32_t al = ah + L::A_BYTES;
             const uint32_t bh = ah + X::kOps * L::A_BYTES;
             const uint32_t bl = bh + L::B_BYTES;
-            wgmma_fence();
 #pragma unroll
             for (int pass = 0; pass < PASSES; ++pass) {
                 const uint32_t aa = pass == 2 ? al : ah, bb = pass == 1 ? bl : bh;
 #pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k)
+                for (int k = 0; k < BK / WGMMA_K; ++k)
                     acc.template mma_halves<0, 0, typename X::Mma>(make_desc(aa + k * 32, 16, 1024), make_desc(aa + 64 * 128 + k * 32, 16, 1024),
                                                                    make_desc(bb + k * 32, 16, 1024), make_desc(bb + 64 * 128 + k * 32, 16, 1024),
                                                                    (i | pass | k) != 0);
             }
-            wgmma_commit();
-            wgmma_wait<1>();
-            if (pending && mt == 0) mbar_arrive_cta(pending);
-            pending = empty + s;
-        }
-        wgmma_wait<0>();
-        if (pending && mt == 0) mbar_arrive_cta(pending);
-        mma_group_sync();
-        acc.store(acc_tile, mt);
-        mma_group_sync();
-        if (mt == 0) mbar_arrive_cta(tmem_full);
+        });
+        mma_publish<BN>(acc, acc_tile, acc_full, mt);
         return;
     }
     reg_dec<64>();
@@ -298,7 +275,7 @@ __device__ __forceinline__ void dcn_fwd_body(const CUtensorMap &tmWh, const CUte
                     }
                 }
                 fence_proxy_async();                          // generic-proxy smem writes -> visible to wgmma
-                mbar_arrive_cta(full + s);
+                mbar_arrive(full + s);
             }
         }
         // ------------------------------------------------------------ epilogue: accumulator tile -> NCHW (+ bias); 4 warps per 32-row quarter
@@ -307,7 +284,7 @@ __device__ __forceinline__ void dcn_fwd_body(const CUtensorMap &tmWh, const CUte
         const int er = q * 32 + lane;
         const int ey = ty0 + (er >> 4), ex = tx0 + (er & 15);
         const int prow = (ey < a.Ho && ex < a.Wo) ? ey * a.Wo + ex : a.P;
-        mbar_wait(tmem_full, 0);
+        mbar_wait(acc_full, 0);
         T *ob = a.out + ((int64_t)b * a.Cout + n0) * a.P + prow;
 #pragma unroll 1
         for (int c = part * (BN / 128); c < (part + 1) * (BN / 128); ++c) {
@@ -379,7 +356,7 @@ __device__ __forceinline__ void dcn_wgrad_body(const CUtensorMap &tmGh, const CU
     uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);         // produced operand: full (512 producer arrivals) / empty (MMA commit)
     uint64_t *empty = full + STAGES;
     uint64_t *a_full = empty + STAGES, *a_empty = a_full + 1;  // TMA operand, single buffer
-    uint64_t *tmem_full = a_empty + 1;
+    uint64_t *acc_full = a_empty + 1;
     float4 *tapw_all = (float4 *)(smem + L::TAP_OFF);         // [STAGES][128]
     uint2 *tapc_all = (uint2 *)(tapw_all + STAGES * BM);      // [STAGES][128]
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -394,7 +371,7 @@ __device__ __forceinline__ void dcn_wgrad_body(const CUtensorMap &tmGh, const CU
         if constexpr (X::kSplit) tma_prefetch_desc(&tmGl);
         for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, kProducerThreads); mbar_init(empty + s, 1); }
         mbar_init(a_full, 1); mbar_init(a_empty, 1);
-        mbar_init(tmem_full, 1);
+        mbar_init(acc_full, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -435,21 +412,21 @@ __device__ __forceinline__ void dcn_wgrad_body(const CUtensorMap &tmGh, const CU
             for (int pass = 0; pass < PASSES; ++pass) {
                 const uint32_t aa = pass == 2 ? al : ah, bb = pass == 1 ? bl : bh;       // Ah Bh, Ah Bl, Al Bh
 #pragma unroll
-                for (int j = 0; j < BM / UMMA_K; ++j) {                                   // 8 steps of 16 pixels
-                    const uint32_t ak = aa + (j >> 2) * (BM * 128) + (j & 3) * 32;
-                    acc.template mma<0, 1, typename X::Mma>(make_desc(ak, 16, 1024), make_desc(ak + 64 * 128, 16, 1024),
-                                                            make_desc(bb + j * 2048, BM * 128, 1024), (i | pass | j) != 0);
+                for (int j = 0; j < BM / WGMMA_K; ++j) {                                   // 8 steps of 16 pixels
+                    const uint32_t ak = aa + (j >> 2) * (BM * 128);                       // 64-pixel atom of the step
+                    acc.template mma<0, 1, typename X::Mma>(desc_kmajor(ak, j & 3), desc_kmajor(ak, j & 3, 1),
+                                                            desc_mnmajor(bb, j, BM * 128), (i | pass | j) != 0);
                 }
             }
             wgmma_commit();
             wgmma_wait<0>();
-            if (mt == 0) { mbar_arrive_cta(empty + s); mbar_arrive_cta(a_empty); }
+            if (mt == 0) { mbar_arrive(empty + s); mbar_arrive(a_empty); }
         }
         if (nt > 0) {
             mma_group_sync();
             acc.store(acc_tile, mt);
             mma_group_sync();
-            if (mt == 0) mbar_arrive_cta(tmem_full);
+            if (mt == 0) mbar_arrive(acc_full);
         }
     } else if (warp >= 2 && threadIdx.x < 64 + kProducerThreads) {
         const int pwp = warp - 2;
@@ -555,7 +532,7 @@ __device__ __forceinline__ void dcn_wgrad_body(const CUtensorMap &tmGh, const CU
                 }
             }
             fence_proxy_async();
-            mbar_arrive_cta(full + s);
+            mbar_arrive(full + s);
             if (prep) tap_store(gt + a.splits, (i + 1) & 1, noh, now, nm);
             asm volatile("bar.sync 1, %0;" ::"n"(kProducerThreads) : "memory");
         }
@@ -563,7 +540,7 @@ __device__ __forceinline__ void dcn_wgrad_body(const CUtensorMap &tmGh, const CU
         const int q = warp & 3, part = (warp - 2) >> 2;
         const int co = co0 + q * 32 + lane;
         if (nt > 0) {
-            mbar_wait(tmem_full, 0);
+            mbar_wait(acc_full, 0);
             uint32_t rr[16];
             acc_ld<16>(acc_tile, AccTile<BN>::LD, q * 32, part * 16, rr);
             if (co < a.Cout) {
@@ -736,7 +713,7 @@ __device__ __forceinline__ void dcn_dgrad_body(const CUtensorMap &tmGh, const CU
                     for (int pass = 0; pass < PASSES; ++pass) {
                         const uint32_t aa = pass == 2 ? al : ah, bb = pass == 1 ? bl : bh;
 #pragma unroll
-                        for (int k4 = 0; k4 < L::KB / UMMA_K; ++k4)
+                        for (int k4 = 0; k4 < L::KB / WGMMA_K; ++k4)
                             acc.template mma_halves<1, 1, typename X::Mma>(
                                 make_desc(aa + k4 * 2048, L::KB * 128, 1024), make_desc(aa + L::KB * 128 + k4 * 2048, L::KB * 128, 1024),
                                 make_desc(bb + k4 * 2048, L::KB * 128, 1024), make_desc(bb + L::KB * 128 + k4 * 2048, L::KB * 128, 1024),
@@ -744,15 +721,15 @@ __device__ __forceinline__ void dcn_dgrad_body(const CUtensorMap &tmGh, const CU
                     }
                     wgmma_commit();
                     wgmma_wait<1>();
-                    if (pending && mt == 0) mbar_arrive_cta(pending);
+                    if (pending && mt == 0) mbar_arrive(pending);
                     pending = empty + s;
                 }
                 wgmma_wait<0>();
-                if (pending && mt == 0) mbar_arrive_cta(pending);
+                if (pending && mt == 0) mbar_arrive(pending);
                 if (n > 0) mbar_wait(acc_empty + (buf ^ 1), ((n - 1) >> 1) & 1);
                 acc.store(acc_tile, mt);
                 mma_group_sync();
-                if (mt == 0) mbar_arrive_cta(acc_full + buf);
+                if (mt == 0) mbar_arrive(acc_full + buf);
             }
         return;
     }
@@ -820,7 +797,7 @@ __device__ __forceinline__ void dcn_dgrad_body(const CUtensorMap &tmGh, const CU
                                      "r"(rr[4 * c4]), "r"(rr[4 * c4 + 1]), "r"(rr[4 * c4 + 2]), "r"(rr[4 * c4 + 3]) : "memory");
                 }
                 asm volatile("bar.sync %0, 128;" ::"r"(1 + q) : "memory");
-                if (lane == 0) mbar_arrive_cta(acc_empty + buf);
+                if (lane == 0) mbar_arrive(acc_empty + buf);
                 // the next tap's table: its three global loads are issued now and consumed after this N block's work
                 const bool prep = part == 0 && h == 0 && kk + a.tap_splits < K;
                 DcnDRaw raw = {0.f, 0.f, 0.f};

@@ -14,6 +14,7 @@
 // a shared-memory tile laid over the drained operand ring.  One 128 x BN output tile (BN <= 128: the accumulator is
 // BN registers per MMA thread) per CTA (grid = tiles x split-K); K loops over 64-element blocks.
 #include "wgmma.cuh"
+#include "lstm_cell.cuh"
 #include <stdlib.h>
 
 namespace {
@@ -29,14 +30,14 @@ struct GemmArgs {
 
 // Epilogue shared by the GEMM and convolution kernels: warps 2..5, accumulator tile -> registers -> (bias, ReLU) -> global.
 template <int BN>
-__device__ __forceinline__ void epilogue_store(const GemmArgs &g, const float *acc, uint64_t *tmem_full, int m0, int n0,
+__device__ __forceinline__ void epilogue_store(const GemmArgs &g, const float *acc, uint64_t *acc_full, int m0, int n0,
                                                int warp, int lane, bool have_acc, int64_t row_override = -2) {
         const int q = warp & 3;                               // 32-row quarter of the tile this warp stores
         // output row of this thread: m0 + tile row, or an explicit row (-1 = none) for tiles that are not row ranges
         const int64_t row = row_override == -2 ? (int64_t)(m0 + q * 32 + lane) : (row_override < 0 ? (int64_t)g.M : row_override);
         const int nkb = have_acc ? 1 : 0;
         if (nkb > 0) {
-            mbar_wait(tmem_full, 0);
+            mbar_wait(acc_full, 0);
         }
         float *Cf = (float *)g.C;
         bf16 *Ch = (bf16 *)g.C;
@@ -97,68 +98,19 @@ __device__ __forceinline__ void epilogue_store(const GemmArgs &g, const float *a
 constexpr int kGemmMma0 = 256;                      // first thread of the MMA warpgroup (warps 6, 7 are padding)
 constexpr int kGemmThreads = kGemmMma0 + kMmaThreads;
 
-// The MMA warpgroup's K loop over the ring: wgmma for stage i is committed, then stage i - 1 is known to have retired and
-// its slot is handed back to the producers.  issue(i, s) queues the wgmmas of one stage.
-template <typename Issue>
-__device__ __forceinline__ void mma_ring(int nkb, int stages, uint64_t *full, uint64_t *empty, bool leader, Issue issue) {
-    uint64_t *pending = nullptr;
-    for (int i = 0; i < nkb; ++i) {
-        const int s = i % stages;
-        mbar_wait(full + s, (i / stages) & 1);
-        wgmma_fence();
-        issue(i, s);
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (pending && leader) mbar_arrive(pending);
-        pending = empty + s;
-    }
-    wgmma_wait<0>();
-    if (pending && leader) mbar_arrive(pending);
-}
-// ... and the hand-over: the ring is drained (every load was consumed), so the accumulator tile is laid over it.
-template <int BN>
-__device__ __forceinline__ void mma_publish(const AccTile<BN> &acc, float *tile, uint64_t *tmem_full, int mt) {
-    mma_group_sync();
-    acc.store(tile, mt);
-    mma_group_sync();
-    if (mt == 0) mbar_arrive(tmem_full);
-}
-
-template <int BN, int STAGES>
-struct SmemLayout {
-    static constexpr int A_BYTES = BM * BK * 2;      // 16 KB
-    static constexpr int B_BYTES = BN * BK * 2;
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
-    static constexpr int TOTAL = BAR_OFF + (2 * STAGES + 1) * 8 + 16 + 1024;   // + alignment slack
-    static_assert(AccTile<BN>::BYTES <= BAR_OFF, "the accumulator tile is laid over the operand ring");
-};
-
 template <int BN, int STAGES, int A_MN, int B_MN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmArgs g) {
-    using L = SmemLayout<BN, STAGES>;
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);   // SW128 needs 1024 B
-    uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
-    uint64_t *empty = full + STAGES;
-    uint64_t *tmem_full = empty + STAGES;
-
+    using L = RingSmem<BN, STAGES>;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
     const int kb_total = (g.K + BK - 1) / BK;
     const int kb_lo = blockIdx.z * g.kblocks_per_split;
     const int kb_hi = min(kb_total, kb_lo + g.kblocks_per_split);
     const int nkb = kb_hi - kb_lo;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmA);
-        tma_prefetch_desc(&tmB);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); }
-        mbar_init(tmem_full, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
+    const Ring rg = ring_init<L>(warp == 0 && lane == 0, 1, [&] { tma_prefetch_desc(&tmA); tma_prefetch_desc(&tmB); });
+    unsigned char *smem = rg.smem;
+    uint64_t *full = rg.full, *empty = rg.empty, *acc_full = rg.acc_full;
     float *acc_tile = (float *)smem;
 
     if (warp == 0) {
@@ -192,22 +144,17 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
             const uint32_t b_addr = a_addr + L::A_BYTES;
 #pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-                // K-major: 8-row groups 1024 B apart (SBO), advance 32 B per 16-deep step inside the 128 B atom; the
-                //          tile's lower 64 rows start 64 * 128 B further on.
-                // MN-major: 64-element M/N atoms BK*128 B apart (LBO), 8-row K groups 1024 B apart (SBO),
-                //           advance 16 rows * 128 B per step; the lower 64 rows are the second atom.
-                const uint64_t a_lo = A_MN == 0 ? make_desc(a_addr + k * 32, 16, 1024) : make_desc(a_addr + k * 2048, BK * 128, 1024);
-                const uint64_t a_hi = A_MN == 0 ? make_desc(a_addr + 64 * 128 + k * 32, 16, 1024)
-                                                : make_desc(a_addr + BK * 128 + k * 2048, BK * 128, 1024);
-                const uint64_t bd = B_MN == 0 ? make_desc(b_addr + k * 32, 16, 1024) : make_desc(b_addr + k * 2048, BK * 128, 1024);
+            for (int k = 0; k < BK / WGMMA_K; ++k) {
+                const uint64_t a_lo = A_MN == 0 ? desc_kmajor(a_addr, k) : desc_mnmajor(a_addr, k, BK * 128);
+                const uint64_t a_hi = A_MN == 0 ? desc_kmajor(a_addr, k, 1) : desc_mnmajor(a_addr, k, BK * 128, 1);
+                const uint64_t bd = B_MN == 0 ? desc_kmajor(b_addr, k) : desc_mnmajor(b_addr, k, BK * 128);
                 acc.template mma<A_MN, B_MN>(a_lo, a_hi, bd, (i | k) != 0);
             }
         });
-        if (nkb > 0) mma_publish<BN>(acc, acc_tile, tmem_full, mt);
+        if (nkb > 0) mma_publish<BN>(acc, acc_tile, acc_full, mt);
     } else if (warp >= 2 && threadIdx.x < 192) {
         // ------------------------------------------------------------ epilogue (warps 2..5)
-        epilogue_store<BN>(g, acc_tile, tmem_full, m0, n0, warp, lane, nkb > 0);
+        epilogue_store<BN>(g, acc_tile, acc_full, m0, n0, warp, lane, nkb > 0);
     }
 }
 
@@ -243,15 +190,6 @@ __device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void *src, 
 
 // One 128-row tile per CTA: a second accumulator would double the MMA warpgroup's register need (BN registers per thread
 // per tile), which is a limit of the one-warpgroup design, not a measured choice.
-template <int BN, int STAGES>
-struct ConvSmem {
-    static constexpr int A_BYTES = BM * BK * 2;
-    static constexpr int B_BYTES = BN * BK * 2;
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
-    static constexpr int TOTAL = BAR_OFF + (2 * STAGES + 1) * 8 + 16 + 1024;
-};
-
 // TMA_A = 1: "same"-padded convolutions whose 128-pixel tiles are whole row segments (W | 128 or 128 | W) fetch the
 // activation tile with ONE 4-D TMA per K block (tap shift = signed coordinate offset, padding = TMA zero fill)
 // instead of 1024 cp.async from the LSU.
@@ -260,13 +198,14 @@ __global__ void __launch_bounds__(kGemmThreads, 1)
 conv_fprop_tcgen05_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmX0,
                           const __grid_constant__ CUtensorMap tmX1, const __grid_constant__ CUtensorMap tmX2,
                           const __grid_constant__ CUtensorMap tmX3, ConvArgs a) {
-    using L = ConvSmem<BN, STAGES>;
-    static_assert(AccTile<BN>::BYTES <= L::BAR_OFF, "the accumulator tile is laid over the operand ring");
+    // The barrier set-up and the segment decode below are spelled out here rather than taken from ring_init and a shared
+    // decode function: through either helper the compiler emits different machine code for the TMA_A instantiations.
+    using L = RingSmem<BN, STAGES>;
     extern __shared__ unsigned char smem_raw[];
     unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
     uint64_t *empty = full + STAGES;
-    uint64_t *tmem_full = empty + STAGES;
+    uint64_t *acc_full = empty + STAGES;
     const GemmArgs &g = a.g;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
@@ -277,7 +216,7 @@ conv_fprop_tcgen05_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_
         tma_prefetch_desc(&tmB);
         if (TMA_A) tma_prefetch_desc(&tmX0);
         for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, TMA_A ? 1 : 1 + 128); mbar_init(empty + s, 1); }
-        mbar_init(tmem_full, 1);
+        mbar_init(acc_full, 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -320,11 +259,10 @@ conv_fprop_tcgen05_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_
             const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
             const uint32_t b_addr = a_addr + L::A_BYTES;
 #pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k)
-                acc.template mma<0, 0>(make_desc(a_addr + k * 32, 16, 1024), make_desc(a_addr + 64 * 128 + k * 32, 16, 1024),
-                                       make_desc(b_addr + k * 32, 16, 1024), (i | k) != 0);
+            for (int k = 0; k < BK / WGMMA_K; ++k)
+                acc.template mma<0, 0>(desc_kmajor(a_addr, k), desc_kmajor(a_addr, k, 1), desc_kmajor(b_addr, k), (i | k) != 0);
         });
-        if (nkb > 0) mma_publish<BN>(acc, acc_tile, tmem_full, mt);
+        if (nkb > 0) mma_publish<BN>(acc, acc_tile, acc_full, mt);
     } else if (warp < 2 || threadIdx.x >= 192) {
         // warp 1 and the padding warps have no role
     } else if (TMA_A) {
@@ -339,7 +277,7 @@ conv_fprop_tcgen05_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_
         const int dw = r % bw, dh = (r / bw) % bh, dn = r / (bw * bh);
         const int pn = nb * a.seg[sel].bn + dn, phh = (lt - nb * a.seg[sel].h_blocks) * bh + dh, pww = a.seg[sel].w0 + dw;
         if (pn < a.N && phh < a.Ho && pww < a.Wo) prow = ((int64_t)pn * a.Ho + phh) * a.Wo + pww;
-        epilogue_store<BN>(g, acc_tile, tmem_full, 0, n0, warp, lane, nkb > 0, prow);
+        epilogue_store<BN>(g, acc_tile, acc_full, 0, n0, warp, lane, nkb > 0, prow);
     } else {
         // ------------------------------------------------------------ activation gather (one thread = one tile row)
         const int r = threadIdx.x - 64;
@@ -378,7 +316,7 @@ conv_fprop_tcgen05_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_
         cp_async_wait<0>();
         fence_proxy_async();
         for (int i = (nkb >= D - 1 ? nkb - (D - 1) : 0); i < nkb; ++i) mbar_arrive(full + i % STAGES);
-        epilogue_store<BN>(g, acc_tile, tmem_full, m0, n0, warp, lane, nkb > 0);
+        epilogue_store<BN>(g, acc_tile, acc_full, m0, n0, warp, lane, nkb > 0);
     }
 }
 
@@ -396,41 +334,22 @@ struct WgradArgs {
     GemmArgs g;                 // M = Cout, N = kh*kw*C, C = dW, atomic = 1
 };
 
-
-template <int BN, int RB, int STAGES>
-struct WgradSmem {
-    static constexpr int A_BYTES = 2 * RB * 128;              // 128 output channels = 2 atoms of [RB rows][128 B]
-    static constexpr int B_BYTES = (BN / 64) * RB * 128;
-    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
-    static constexpr int TOTAL = BAR_OFF + (2 * STAGES + 1) * 8 + 16 + 1024;
-};
+// A: 128 output channels = 2 atoms of [RB rows][128 B]; B: BN / 64 atoms
+template <int BN, int RB, int STAGES> using WgradSmem = RingSmem<BN, STAGES, 2 * RB * 128, (BN / 64) * RB * 128>;
 
 template <int BN, int RB, int STAGES>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 conv_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant__ CUtensorMap tmX, WgradArgs a) {
     using L = WgradSmem<BN, RB, STAGES>;
-    static_assert(AccTile<BN>::BYTES <= L::BAR_OFF, "the accumulator tile is laid over the operand ring");
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
-    uint64_t *empty = full + STAGES;
-    uint64_t *tmem_full = empty + STAGES;
     const GemmArgs &g = a.g;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
     const int kb_lo = blockIdx.z * a.kblocks_per_split;
     const int kb_hi = min(a.kb_total, kb_lo + a.kblocks_per_split);
     const int nkb = kb_hi - kb_lo;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&tmDz);
-        tma_prefetch_desc(&tmX);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); }
-        mbar_init(tmem_full, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
+    const Ring rg = ring_init<L>(warp == 0 && lane == 0, 1, [&] { tma_prefetch_desc(&tmDz); tma_prefetch_desc(&tmX); });
+    unsigned char *smem = rg.smem;
+    uint64_t *full = rg.full, *empty = rg.empty, *acc_full = rg.acc_full;
     float *acc_tile = (float *)smem;
 
     if (warp == 0) {
@@ -475,13 +394,13 @@ conv_wgrad_tcgen05_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid
             const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
             const uint32_t b_addr = a_addr + L::A_BYTES;
 #pragma unroll
-            for (int k = 0; k < RB / UMMA_K; ++k)
-                acc.template mma<1, 1>(make_desc(a_addr + k * 2048, RB * 128, 1024), make_desc(a_addr + RB * 128 + k * 2048, RB * 128, 1024),
-                                       make_desc(b_addr + k * 2048, RB * 128, 1024), (i | k) != 0);
+            for (int k = 0; k < RB / WGMMA_K; ++k)
+                acc.template mma<1, 1>(desc_mnmajor(a_addr, k, RB * 128), desc_mnmajor(a_addr, k, RB * 128, 1),
+                                       desc_mnmajor(b_addr, k, RB * 128), (i | k) != 0);
         });
-        if (nkb > 0) mma_publish<BN>(acc, acc_tile, tmem_full, mt);
+        if (nkb > 0) mma_publish<BN>(acc, acc_tile, acc_full, mt);
     } else if (warp >= 2 && threadIdx.x < 192) {
-        epilogue_store<BN>(g, acc_tile, tmem_full, m0, n0, warp, lane, nkb > 0);
+        epilogue_store<BN>(g, acc_tile, acc_full, m0, n0, warp, lane, nkb > 0);
     }
 }
 
@@ -515,12 +434,7 @@ lstm_step_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
                              const __grid_constant__ CUtensorMap tmB0, const __grid_constant__ CUtensorMap tmB1,
                              LstmFwdArgs a) {
     constexpr int BN = kLstmBN;
-    using L = SmemLayout<BN, STAGES>;
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
-    uint64_t *empty = full + STAGES;
-    uint64_t *tmem_full = empty + STAGES;
+    using L = RingSmem<BN, STAGES>;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dir = blockIdx.z;
     const CUtensorMap *tmA = dir ? &tmA1 : &tmA0;
@@ -528,15 +442,9 @@ lstm_step_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
     const LstmFwdDir &q = a.d[dir];
     const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
     const int nkb = a.have_h ? a.H / BK : 0;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(tmA);
-        tma_prefetch_desc(tmB);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); }
-        mbar_init(tmem_full, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
+    const Ring rg = ring_init<L>(warp == 0 && lane == 0, 1, [&] { tma_prefetch_desc(tmA); tma_prefetch_desc(tmB); });
+    unsigned char *smem = rg.smem;
+    uint64_t *full = rg.full, *empty = rg.empty, *acc_full = rg.acc_full;
     float *acc_tile = (float *)smem;
 
     if (warp == 0) {
@@ -557,15 +465,14 @@ lstm_step_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
             const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
             const uint32_t b_addr = a_addr + L::A_BYTES;
 #pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k)
-                acc.template mma<0, 0>(make_desc(a_addr + k * 32, 16, 1024), make_desc(a_addr + 64 * 128 + k * 32, 16, 1024),
-                                       make_desc(b_addr + k * 32, 16, 1024), (i | k) != 0);
+            for (int k = 0; k < BK / WGMMA_K; ++k)
+                acc.template mma<0, 0>(desc_kmajor(a_addr, k), desc_kmajor(a_addr, k, 1), desc_kmajor(b_addr, k), (i | k) != 0);
         });
-        if (nkb > 0) mma_publish<BN>(acc, acc_tile, tmem_full, mt);
+        if (nkb > 0) mma_publish<BN>(acc, acc_tile, acc_full, mt);
     } else if (warp >= 2 && threadIdx.x < 64 + 16 * 32) {
         const int qd = warp & 3, grp = (warp - 2) >> 2;       // 32-row quarter of the tile, 16-column group
         const int row = m0 + qd * 32 + lane;
-        if (nkb > 0) mbar_wait(tmem_full, 0);
+        if (nkb > 0) mbar_wait(acc_full, 0);
         const int H = a.H;
         uint32_t r[16];
         if (nkb > 0) acc_ld<16>(acc_tile, AccTile<BN>::LD, qd * 32, grp * 16, r);
@@ -603,13 +510,13 @@ lstm_step_fwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
             float act[16], cn[4], hn[4];
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
-                const float i_ = sigmoid_fast(pre[4 * u] + __uint_as_float(r[4 * u]) + bb[4 * u]);
-                const float f_ = sigmoid_fast(pre[4 * u + 1] + __uint_as_float(r[4 * u + 1]) + bb[4 * u + 1]);
-                const float g_ = tanh_fast(pre[4 * u + 2] + __uint_as_float(r[4 * u + 2]) + bb[4 * u + 2]);
-                const float o_ = sigmoid_fast(pre[4 * u + 3] + __uint_as_float(r[4 * u + 3]) + bb[4 * u + 3]);
-                cn[u] = f_ * cpv[u] + i_ * g_;
-                hn[u] = o_ * tanh_fast(cn[u]);
-                act[4 * u] = i_; act[4 * u + 1] = f_; act[4 * u + 2] = g_; act[4 * u + 3] = o_;
+                const LstmUnit c = lstm_unit_fwd<CellFast>(
+                    pre[4 * u] + __uint_as_float(r[4 * u]) + bb[4 * u], pre[4 * u + 1] + __uint_as_float(r[4 * u + 1]) + bb[4 * u + 1],
+                    pre[4 * u + 2] + __uint_as_float(r[4 * u + 2]) + bb[4 * u + 2], pre[4 * u + 3] + __uint_as_float(r[4 * u + 3]) + bb[4 * u + 3],
+                    cpv[u]);
+                cn[u] = c.c;
+                hn[u] = c.h;
+                act[4 * u] = c.i; act[4 * u + 1] = c.f; act[4 * u + 2] = c.g; act[4 * u + 3] = c.o;
             }
 #pragma unroll
             for (int v = 0; v < 2; ++v) {
@@ -646,12 +553,7 @@ lstm_step_bwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
                              const __grid_constant__ CUtensorMap tmB0, const __grid_constant__ CUtensorMap tmB1,
                              LstmBwdArgs a) {
     constexpr int BN = kLstmBN;     // 64 hidden units per CTA
-    using L = SmemLayout<BN, STAGES>;
-    extern __shared__ unsigned char smem_raw[];
-    unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
-    uint64_t *empty = full + STAGES;
-    uint64_t *tmem_full = empty + STAGES;
+    using L = RingSmem<BN, STAGES>;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dir = blockIdx.z;
     const CUtensorMap *tmA = dir ? &tmA1 : &tmA0;
@@ -659,15 +561,9 @@ lstm_step_bwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
     const LstmBwdDir &q = a.d[dir];
     const int m0 = blockIdx.x * BM, n0 = blockIdx.y * BN;
     const int nkb = a.have_rec ? (4 * a.H) / BK : 0;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(tmA);
-        tma_prefetch_desc(tmB);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); }
-        mbar_init(tmem_full, 1);
-        fence_barrier_init();
-    }
-    __syncthreads();
+    const Ring rg = ring_init<L>(warp == 0 && lane == 0, 1, [&] { tma_prefetch_desc(tmA); tma_prefetch_desc(tmB); });
+    unsigned char *smem = rg.smem;
+    uint64_t *full = rg.full, *empty = rg.empty, *acc_full = rg.acc_full;
     float *acc_tile = (float *)smem;
 
     if (warp == 0) {
@@ -688,15 +584,14 @@ lstm_step_bwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
             const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES);
             const uint32_t b_addr = a_addr + L::A_BYTES;
 #pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k)
-                acc.template mma<0, 1>(make_desc(a_addr + k * 32, 16, 1024), make_desc(a_addr + 64 * 128 + k * 32, 16, 1024),
-                                       make_desc(b_addr + k * 2048, BK * 128, 1024), (i | k) != 0);
+            for (int k = 0; k < BK / WGMMA_K; ++k)
+                acc.template mma<0, 1>(desc_kmajor(a_addr, k), desc_kmajor(a_addr, k, 1), desc_mnmajor(b_addr, k, BK * 128), (i | k) != 0);
         });
-        if (nkb > 0) mma_publish<BN>(acc, acc_tile, tmem_full, mt);
+        if (nkb > 0) mma_publish<BN>(acc, acc_tile, acc_full, mt);
     } else if (warp >= 2 && threadIdx.x < 64 + 16 * 32) {
         const int qd = warp & 3, grp = (warp - 2) >> 2;
         const int row = m0 + qd * 32 + lane;
-        if (nkb > 0) mbar_wait(tmem_full, 0);
+        if (nkb > 0) mbar_wait(acc_full, 0);
         const int H = a.H;
         uint32_t r[16];
         if (nkb > 0) acc_ld<16>(acc_tile, AccTile<BN>::LD, qd * 32, grp * 16, r);
@@ -739,15 +634,13 @@ lstm_step_bwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
                         const int uu = h * 2 + w2;             // unit inside this group of 8
                         const float2 fi = __bfloat1622float2(g2[2 * w2]);       // (i, f)
                         const float2 fg = __bfloat1622float2(g2[2 * w2 + 1]);   // (g, o)
-                        const float i_ = fi.x, f_ = fi.y, g_ = fg.x, o_ = fg.y;
-                        const float dh = dyf[uu] + __uint_as_float(r[v * 8 + uu]);
-                        const float tc = tanh_fast(cf[uu]);
-                        const float dct = dcf[uu] + dh * o_ * (1.f - tc * tc);
-                        dgf[uu * 4] = dct * g_ * i_ * (1.f - i_);
-                        dgf[uu * 4 + 1] = dct * cpf[uu] * f_ * (1.f - f_);
-                        dgf[uu * 4 + 2] = dct * i_ * (1.f - g_ * g_);
-                        dgf[uu * 4 + 3] = dh * tc * o_ * (1.f - o_);
-                        dcf[uu] = dct * f_;
+                        const LstmUnitGrad d = lstm_unit_bwd<CellFast>(fi.x, fi.y, fg.x, fg.y, cf[uu], cpf[uu],
+                                                                       dyf[uu] + __uint_as_float(r[v * 8 + uu]), dcf[uu]);
+                        dgf[uu * 4] = d.di;
+                        dgf[uu * 4 + 1] = d.df;
+                        dgf[uu * 4 + 2] = d.dg;
+                        dgf[uu * 4 + 3] = d.do_;
+                        dcf[uu] = d.dc_prev;
                     }
                 }
 #pragma unroll
@@ -766,14 +659,21 @@ lstm_step_bwd_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA0, const __g
     }
 }
 
+// Opts kern into `smem` bytes of dynamic shared memory, launches it and checks the launch; attr_where / where name the
+// failing step in the error.
+template <typename... P, typename... A>
+int launch_kernel(void (*kern)(P...), dim3 grid, int threads, int smem, cudaStream_t st, const char *attr_where,
+                  const char *where, const A &...args) {
+    { int rc_attr = ensure_dyn_smem((const void *)kern, smem, attr_where); if (rc_attr) return rc_attr; }
+    kern<<<grid, threads, smem, st>>>(args...);
+    return check_launch(where);
+}
+
 template <int BN, int STAGES, int A_MN, int B_MN>
 int launch(const CUtensorMap &ta, const CUtensorMap &tb, const GemmArgs &g, int splits, cudaStream_t st) {
-    using L = SmemLayout<BN, STAGES>;
-    auto kern = gemm_tcgen05_kernel<BN, STAGES, A_MN, B_MN>;
-    { int rc_attr = ensure_dyn_smem((const void *)kern, L::TOTAL, "gemm_tcgen05 smem attr"); if (rc_attr) return rc_attr; }
     dim3 grid((unsigned)ceil_div(g.M, BM), (unsigned)ceil_div(g.N, BN), (unsigned)splits);
-    kern<<<grid, kGemmThreads, L::TOTAL, st>>>(ta, tb, g);
-    return check_launch("gemm_tcgen05_kernel");
+    return launch_kernel(gemm_tcgen05_kernel<BN, STAGES, A_MN, B_MN>, grid, kGemmThreads, RingSmem<BN, STAGES>::TOTAL, st,
+                         "gemm_tcgen05 smem attr", "gemm_tcgen05_kernel", ta, tb, g);
 }
 
 // 4-D bf16 NHWC tensor map {C, W, H, N}, box {64, box_w, 1, 1}
@@ -797,22 +697,16 @@ int make_map_nhwc(CUtensorMap *m, const void *base, int64_t C, int64_t W, int64_
 
 template <int BN, int STAGES, int TMA_A>
 int launch_conv(const CUtensorMap &tb, const CUtensorMap *tx, const ConvArgs &a, int tiles, cudaStream_t st) {
-    using L = ConvSmem<BN, STAGES>;
-    auto kern = conv_fprop_tcgen05_kernel<BN, STAGES, TMA_A>;
-    { int rc_attr = ensure_dyn_smem((const void *)kern, L::TOTAL, "conv_fprop smem attr"); if (rc_attr) return rc_attr; }
     dim3 grid(TMA_A ? (unsigned)tiles : (unsigned)ceil_div(a.g.M, BM), (unsigned)ceil_div(a.g.N, BN), 1);
-    kern<<<grid, kGemmThreads, L::TOTAL, st>>>(tb, tx[0], tx[1], tx[2], tx[3], a);
-    return check_launch("conv_fprop_tcgen05_kernel");
+    return launch_kernel(conv_fprop_tcgen05_kernel<BN, STAGES, TMA_A>, grid, kGemmThreads, RingSmem<BN, STAGES>::TOTAL, st,
+                         "conv_fprop smem attr", "conv_fprop_tcgen05_kernel", tb, tx[0], tx[1], tx[2], tx[3], a);
 }
 
 template <int BN, int RB, int STAGES>
 int launch_wgrad(const CUtensorMap &tdz, const CUtensorMap &tx, const WgradArgs &a, int splits, cudaStream_t st) {
-    using L = WgradSmem<BN, RB, STAGES>;
-    auto kern = conv_wgrad_tcgen05_kernel<BN, RB, STAGES>;
-    { int rc_attr = ensure_dyn_smem((const void *)kern, L::TOTAL, "conv_wgrad smem attr"); if (rc_attr) return rc_attr; }
     dim3 grid((unsigned)ceil_div(a.g.M, BM), (unsigned)ceil_div(a.g.N, BN), (unsigned)splits);
-    kern<<<grid, kGemmThreads, L::TOTAL, st>>>(tdz, tx, a);
-    return check_launch("conv_wgrad_tcgen05_kernel");
+    return launch_kernel(conv_wgrad_tcgen05_kernel<BN, RB, STAGES>, grid, kGemmThreads, WgradSmem<BN, RB, STAGES>::TOTAL, st,
+                         "conv_wgrad smem attr", "conv_wgrad_tcgen05_kernel", tdz, tx, a);
 }
 
 }  // namespace
@@ -1020,12 +914,9 @@ int mr_lstm_step_fwd_tcgen05(const void *const *h_prev, const void *const *Whh, 
         a.d[d].gates = (bf16 *)gates[d]; a.d[d].bias = bias[d]; a.d[d].c_prev = c_prev[d]; a.d[d].c_out = c_out[d];
         a.d[d].h_out = (bf16 *)h_out[d]; a.d[d].h_next = (bf16 *)h_next[d];
     }
-    using L = SmemLayout<kLstmBN, 4>;
-    auto kern = lstm_step_fwd_tcgen05_kernel<4>;
-    { int rc_attr = ensure_dyn_smem((const void *)kern, L::TOTAL, "lstm fwd smem attr"); if (rc_attr) return rc_attr; }
     dim3 grid((unsigned)ceil_div(B, BM), (unsigned)(4 * H / kLstmBN), 2);
-    kern<<<grid, kLstmThreads, L::TOTAL, (cudaStream_t)stream>>>(ta[0], ta[1], tb[0], tb[1], a);
-    return check_launch("lstm_step_fwd_tcgen05_kernel");
+    return launch_kernel(lstm_step_fwd_tcgen05_kernel<4>, grid, kLstmThreads, RingSmem<kLstmBN, 4>::TOTAL, (cudaStream_t)stream,
+                         "lstm fwd smem attr", "lstm_step_fwd_tcgen05_kernel", ta[0], ta[1], tb[0], tb[1], a);
 }
 
 /* dG_next[d]: [B,4H] bf16 gate gradients of the step processed before this one (ignored when have_rec == 0). */
@@ -1045,12 +936,9 @@ int mr_lstm_step_bwd_tcgen05(const void *const *dG_next, const void *const *Whh,
         a.d[d].gates = (const bf16 *)gates[d]; a.d[d].c = c[d]; a.d[d].c_prev = c_prev[d];
         a.d[d].dh_out = (const bf16 *)dh_out[d]; a.d[d].dc = dc[d]; a.d[d].dgates = (bf16 *)dgates[d];
     }
-    using L = SmemLayout<kLstmBN, 6>;
-    auto kern = lstm_step_bwd_tcgen05_kernel<6>;
-    { int rc_attr = ensure_dyn_smem((const void *)kern, L::TOTAL, "lstm bwd smem attr"); if (rc_attr) return rc_attr; }
     dim3 grid((unsigned)ceil_div(B, BM), (unsigned)(H / kLstmBN), 2);
-    kern<<<grid, kLstmThreads, L::TOTAL, (cudaStream_t)stream>>>(ta[0], ta[1], tb[0], tb[1], a);
-    return check_launch("lstm_step_bwd_tcgen05_kernel");
+    return launch_kernel(lstm_step_bwd_tcgen05_kernel<6>, grid, kLstmThreads, RingSmem<kLstmBN, 6>::TOTAL, (cudaStream_t)stream,
+                         "lstm bwd smem attr", "lstm_step_bwd_tcgen05_kernel", ta[0], ta[1], tb[0], tb[1], a);
 }
 
 }  // extern "C"

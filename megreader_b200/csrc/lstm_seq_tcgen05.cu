@@ -17,6 +17,7 @@
 // Every wait is bounded: on timeout the CTA records an error word (flags[2*row_tiles]) and runs to completion with
 // undefined results instead of hanging the device.
 #include "wgmma.cuh"
+#include "lstm_cell.cuh"
 #include <stdlib.h>
 
 namespace {
@@ -115,8 +116,8 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
     float *acc_tile = (float *)(Ct + 8192);               // [128 rows x (64 + 1)] fp32      recurrent product of this step
     uint64_t *wfull = (uint64_t *)(Ct + 8192 + AccTile<kBN>::BYTES);
     uint64_t *afull = wfull + 1;                          // [8]
-    uint64_t *tmem_full = afull + 8;
-    uint64_t *gfull = tmem_full + 1;                      // [2]
+    uint64_t *acc_full = afull + 8;
+    uint64_t *gfull = acc_full + 1;                       // [2]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int dir = blockIdx.z;
@@ -135,7 +136,7 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
         tma_prefetch_desc(&tmC3);
         mbar_init(wfull, 1);
         for (int i = 0; i < 8; ++i) mbar_init(afull + i, 1);
-        mbar_init(tmem_full, 1);
+        mbar_init(acc_full, 1);
         mbar_init(gfull, 1);
         mbar_init(gfull + 1, 1);
         fence_barrier_init();
@@ -169,16 +170,15 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
                 const uint32_t a_addr = smem_u32(As + kb * 16384), b_addr = smem_u32(Ws + kb * 8192);
                 wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k)
-                    acc.mma<0, 0>(make_desc(a_addr + k * 32, 16, 1024), make_desc(a_addr + 64 * 128 + k * 32, 16, 1024),
-                                  make_desc(b_addr + k * 32, 16, 1024), (kb | k) != 0);
+                for (int k = 0; k < BK / WGMMA_K; ++k)
+                    acc.mma<0, 0>(desc_kmajor(a_addr, k), desc_kmajor(a_addr, k, 1), desc_kmajor(b_addr, k), (kb | k) != 0);
                 wgmma_commit();
             }
             wgmma_wait<0>();
             // the epilogue warps drained the previous step's tile before any peer could post the arrival this step waited for
             acc.store(acc_tile, mt);
             mma_group_sync();
-            if (mt == 0) { mbar_arrive(tmem_full); MR_TRACE(s, 2); }
+            if (mt == 0) { mbar_arrive(acc_full); MR_TRACE(s, 2); }
         }
     } else if (warp >= 2 && threadIdx.x < 64 + kEpiThreads) {
         if (threadIdx.x != 64) trace = nullptr;
@@ -216,7 +216,7 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
             pk[1] = *reinterpret_cast<const uint4 *>(gt + swz(rl, 2 * grp + 1));
             uint32_t r[16];
             if (s > 0) {
-                if (!mbar_wait_bounded(tmem_full, (s - 1) & 1, err)) atomicExch(err, 4u);
+                if (!mbar_wait_bounded(acc_full, (s - 1) & 1, err)) atomicExch(err, 4u);
                 acc_ld<16>(acc_tile, AccTile<kBN>::LD, qd * 32, grp * 16, r);
             } else {
 #pragma unroll
@@ -241,13 +241,13 @@ lstm_seq_fwd_kernel(const __grid_constant__ CUtensorMap tmY, const __grid_consta
                 float hn[4];
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
-                    const float i_ = sigmoid_fast(pre[4 * u] + __uint_as_float(r[4 * u]) + bb[4 * u]);
-                    const float f_ = sigmoid_fast(pre[4 * u + 1] + __uint_as_float(r[4 * u + 1]) + bb[4 * u + 1]);
-                    const float g_ = tanh_fast(pre[4 * u + 2] + __uint_as_float(r[4 * u + 2]) + bb[4 * u + 2]);
-                    const float o_ = sigmoid_fast(pre[4 * u + 3] + __uint_as_float(r[4 * u + 3]) + bb[4 * u + 3]);
-                    cst[u] = f_ * cst[u] + i_ * g_;
-                    hn[u] = o_ * tanh_fast(cst[u]);
-                    act[4 * u] = i_; act[4 * u + 1] = f_; act[4 * u + 2] = g_; act[4 * u + 3] = o_;
+                    const LstmUnit c = lstm_unit_fwd<CellFast>(
+                        pre[4 * u] + __uint_as_float(r[4 * u]) + bb[4 * u], pre[4 * u + 1] + __uint_as_float(r[4 * u + 1]) + bb[4 * u + 1],
+                        pre[4 * u + 2] + __uint_as_float(r[4 * u + 2]) + bb[4 * u + 2], pre[4 * u + 3] + __uint_as_float(r[4 * u + 3]) + bb[4 * u + 3],
+                        cst[u]);
+                    cst[u] = c.c;
+                    hn[u] = c.h;
+                    act[4 * u] = c.i; act[4 * u + 1] = c.f; act[4 * u + 2] = c.g; act[4 * u + 3] = c.o;
                 }
                 uint2 hp;
                 __nv_bfloat162 *hh = reinterpret_cast<__nv_bfloat162 *>(&hp);
@@ -324,8 +324,8 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
     uint64_t *wfull = (uint64_t *)(Ws + nkb * kBwdWTile + AccTile<kBwdBN>::BYTES);
     uint64_t *full = wfull + 1;
     uint64_t *empty = full + STAGES;
-    uint64_t *tmem_full = empty + STAGES;
-    uint64_t *gfull = tmem_full + 1;
+    uint64_t *acc_full = empty + STAGES;
+    uint64_t *gfull = acc_full + 1;
     uint64_t *cfull = gfull + 1;                          // [2]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -346,7 +346,7 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
         tma_prefetch_desc(&tmC3);
         mbar_init(wfull, 1);
         for (int i = 0; i < STAGES; ++i) { mbar_init(full + i, 1); mbar_init(empty + i, 1); }
-        mbar_init(tmem_full, 1);
+        mbar_init(acc_full, 1);
         mbar_init(gfull, 1);
         mbar_init(cfull, 1);
         mbar_init(cfull + 1, 1);
@@ -390,9 +390,8 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
                 const uint32_t a_addr = smem_u32(As + s * 16384), b_addr = smem_u32(Ws + kb * kBwdWTile);
                 wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < BK / UMMA_K; ++k)
-                    acc.mma<0, 0>(make_desc(a_addr + k * 32, 16, 1024), make_desc(a_addr + 64 * 128 + k * 32, 16, 1024),
-                                  make_desc(b_addr + k * 32, 16, 1024), (kb | k) != 0);
+                for (int k = 0; k < BK / WGMMA_K; ++k)
+                    acc.mma<0, 0>(desc_kmajor(a_addr, k), desc_kmajor(a_addr, k, 1), desc_kmajor(b_addr, k), (kb | k) != 0);
                 wgmma_commit();
                 wgmma_wait<1>();                                 // the previous k-block has retired: its slot is free
                 if (pending && mt == 0) mbar_arrive(pending);
@@ -402,7 +401,7 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
             if (pending && mt == 0) mbar_arrive(pending);
             acc.store(acc_tile, mt);
             mma_group_sync();
-            if (mt == 0) { mbar_arrive(tmem_full); MR_TRACE(u, 2); }
+            if (mt == 0) { mbar_arrive(acc_full); MR_TRACE(u, 2); }
         }
     } else if (warp >= 2 && threadIdx.x < 64 + kEpiThreads) {
         const bool leader = threadIdx.x == 64;
@@ -454,7 +453,7 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
             }
             uint32_t r[8];
             if (u > 0) {
-                if (!mbar_wait_bounded(tmem_full, (u - 1) & 1, err)) atomicExch(err, 4u);
+                if (!mbar_wait_bounded(acc_full, (u - 1) & 1, err)) atomicExch(err, 4u);
                 acc_ld<8>(acc_tile, AccTile<kBwdBN>::LD, qd * 32, grp * 8, r);
             } else {
 #pragma unroll
@@ -477,15 +476,13 @@ lstm_seq_bwd_kernel(const __grid_constant__ CUtensorMap tmDG, const __grid_const
                         const int uu = h * 2 + w2;
                         const float2 fi = __bfloat1622float2(g2[2 * w2]);
                         const float2 fg = __bfloat1622float2(g2[2 * w2 + 1]);
-                        const float i_ = fi.x, f_ = fi.y, g_ = fg.x, o_ = fg.y;
-                        const float dh = dyf[uu] + __uint_as_float(r[uu]);
-                        const float tc = tanh_fast(cf[uu]);
-                        const float dct = dcs[uu] + dh * o_ * (1.f - tc * tc);
-                        dgf[w2 * 4] = dct * g_ * i_ * (1.f - i_);
-                        dgf[w2 * 4 + 1] = dct * cpf[uu] * f_ * (1.f - f_);
-                        dgf[w2 * 4 + 2] = dct * i_ * (1.f - g_ * g_);
-                        dgf[w2 * 4 + 3] = dh * tc * o_ * (1.f - o_);
-                        dcs[uu] = dct * f_;
+                        const LstmUnitGrad d = lstm_unit_bwd<CellFast>(fi.x, fi.y, fg.x, fg.y, cf[uu], cpf[uu],
+                                                                       dyf[uu] + __uint_as_float(r[uu]), dcs[uu]);
+                        dgf[w2 * 4] = d.di;
+                        dgf[w2 * 4 + 1] = d.df;
+                        dgf[w2 * 4 + 2] = d.dg;
+                        dgf[w2 * 4 + 3] = d.do_;
+                        dcs[uu] = d.dc_prev;
                     }
                     uint4 o4;
                     __nv_bfloat162 *p2 = reinterpret_cast<__nv_bfloat162 *>(&o4);

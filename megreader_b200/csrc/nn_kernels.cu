@@ -11,6 +11,7 @@
 //
 // dtype codes: 0 = float32, 1 = bfloat16.  "rows" = N*H*W pixels, C = channels (innermost).
 #include "common.cuh"
+#include "lstm_cell.cuh"
 #include <cuda_bf16.h>
 #include <math.h>
 #include <algorithm>
@@ -1077,18 +1078,9 @@ __global__ void gate_rows_permute_kernel(const float *__restrict__ a, const floa
 // layer advance in lock-step, so their cell updates share a launch.
 // gates_pre [B, 4H] (T): x-projection + h_{t-1} W_hh^T already summed by the GEMMs; bias_ih + bias_hh added here.
 // Writes the activated gates back in place (saved for backward), c_t [B,H] fp32, h_t [B,H] (T) into `h_out` (row
-// stride ldh, so it lands directly in the [T, B, 2H] output of the bidirectional layer).
-// bf16 mode uses MUFU.TANH (tanh.approx, ~2^-11 relative error, below bf16 resolution); fp32 mode keeps expf/tanhf
-// so that the parity path stays within 1e-4 of the reference.
-template <typename T> struct CellMath;
-template <> struct CellMath<float> {
-    static __device__ __forceinline__ float th(float x) { return tanhf(x); }
-    static __device__ __forceinline__ float sg(float x) { return 1.f / (1.f + expf(-x)); }
-};
-template <> struct CellMath<bf16> {
-    static __device__ __forceinline__ float th(float x) { float y; asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-    static __device__ __forceinline__ float sg(float x) { return fmaf(0.5f, th(0.5f * x), 0.5f); }
-};
+// stride ldh, so it lands directly in the [T, B, 2H] output of the bidirectional layer).  Activations: CellMath<T>
+// (lstm_cell.cuh).  The cell arithmetic is written out here instead of calling lstm_unit_fwd / lstm_unit_bwd: through
+// those functions the compiler orders these kernels' loads differently and emits different machine code.
 
 struct CellFwdDir { void *gates; const float *b_ih, *b_hh, *c_prev; float *c_out; void *h_out, *h_state; };
 struct CellFwdArgs { CellFwdDir d[2]; int64_t ldh; int B, H; };

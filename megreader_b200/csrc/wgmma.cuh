@@ -1,7 +1,8 @@
-// Shared sm_90a building blocks: PTX wrappers for mbarrier / TMA / wgmma, the shared-memory matrix descriptor, the
-// accumulator hand-over from the MMA warpgroup to the epilogue warps, MUFU-based activations, and host-side tensor-map
-// construction through the driver entry point (no libcuda link dependency).  Included by gemm_tcgen05.cu,
-// lstm_seq_tcgen05.cu and dcn_tcgen05.cu (the file names predate the Hopper port; nothing in them is tcgen05 any more).
+// Shared sm_90a building blocks: PTX wrappers for mbarrier / TMA / wgmma, the shared-memory matrix descriptors, the
+// operand ring of the one-shot kernels (layout, barriers, the MMA warpgroup's K loop), the accumulator hand-over from
+// the MMA warpgroup to the epilogue warps, and host-side tensor-map construction through the driver entry point (no
+// libcuda link dependency).  Included by gemm_tcgen05.cu, lstm_seq_tcgen05.cu and dcn_tcgen05.cu (the file names
+// predate the Hopper port; nothing in them is tcgen05 any more).
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -15,7 +16,7 @@ typedef __nv_bfloat16 bf16;
 
 constexpr int BM = 128;
 constexpr int BK = 64;             // 64 bf16 = 128 bytes = one swizzle atom
-constexpr int UMMA_K = 16;           // K depth of one wgmma instruction (bf16)
+constexpr int WGMMA_K = 16;        // K depth of one wgmma instruction (16-bit operands)
 constexpr int kMmaThreads = 128;    // one warpgroup
 
 // ---------------------------------------------------------------- PTX wrappers
@@ -203,10 +204,85 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes
     return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) |
            ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 62);
 }
+// Descriptors of the 16-deep K step k of a 128-byte-swizzled operand tile at shared address `tile`; 8-row groups are
+// 1024 B apart (SBO).  half = 1 addresses rows (or columns) 64.. of a 128-wide tile.
+// K-major: 128-byte rows; the step starts 32 B further into the swizzle atom, the second half 64 rows * 128 B on.
+__device__ __forceinline__ uint64_t desc_kmajor(uint32_t tile, int k, int half = 0) {
+    return make_desc(tile + half * (64 * 128) + k * 32, 16, 1024);
+}
+// MN-major: 64-element MN atoms `atom` bytes apart (LBO); the step starts 16 K rows * 128 B on, the second half is the
+// second atom.
+__device__ __forceinline__ uint64_t desc_mnmajor(uint32_t tile, int k, uint32_t atom, int half = 0) {
+    return make_desc(tile + half * atom + k * 2048, atom, 1024);
+}
 
-// MUFU.TANH: one instruction, ~2^-11 relative error -- far below bf16 resolution of the stored activations
-__device__ __forceinline__ float tanh_fast(float x) { float y; asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(0.5f, tanh_fast(0.5f * x), 0.5f); }
+// ---------------------------------------------------------------- operand ring of the one-shot kernels
+// STAGES x (A tile, B tile) from a 1024-byte aligned base, then the barriers full[STAGES], empty[STAGES], acc_full.
+// When the K loop is over the accumulator tile is laid over the drained ring.
+template <int BN, int STAGES_, int A_BYTES_ = BM * BK * 2, int B_BYTES_ = BN * BK * 2>
+struct RingSmem {
+    static constexpr int STAGES = STAGES_;
+    static constexpr int A_BYTES = A_BYTES_;
+    static constexpr int B_BYTES = B_BYTES_;
+    static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
+    static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+    static constexpr int TOTAL = BAR_OFF + (2 * STAGES + 1) * 8 + 16 + 1024;   // + alignment slack
+    static_assert(AccTile<BN>::BYTES <= BAR_OFF, "the accumulator tile is laid over the operand ring");
+};
+
+struct Ring {
+    unsigned char *smem;        // the dynamic shared memory, 1024-byte aligned (the 128-byte swizzle needs it)
+    uint64_t *full, *empty;     // [STAGES] each: stage loaded (TMA bytes + full_arrivals) / stage consumed (MMA warpgroup)
+    uint64_t *acc_full;         // the accumulator tile is published
+};
+// Carves the barriers out at L::BAR_OFF (L: the layout, with STAGES and BAR_OFF) and initialises them; the one thread with
+// init = true (warp 0, lane 0: the caller's own expression, which keeps the machine code of its kernel) first runs
+// prefetch(), the tensor-map prefetches.  Every thread of the CTA must call it.
+template <typename L, typename Prefetch>
+__device__ __forceinline__ Ring ring_init(bool init, uint32_t full_arrivals, Prefetch prefetch) {
+    constexpr int STAGES = L::STAGES;
+    extern __shared__ unsigned char smem_raw[];
+    Ring r;
+    r.smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    r.full = (uint64_t *)(r.smem + L::BAR_OFF);
+    r.empty = r.full + STAGES;
+    r.acc_full = r.empty + STAGES;
+    if (init) {
+        prefetch();
+        for (int s = 0; s < STAGES; ++s) { mbar_init(r.full + s, full_arrivals); mbar_init(r.empty + s, 1); }
+        mbar_init(r.acc_full, 1);
+        fence_barrier_init();
+    }
+    __syncthreads();
+    return r;
+}
+
+// The MMA warpgroup's K loop over the ring: the wgmmas of block i are committed, then block i - 1 is known to have
+// retired and its slot is handed back to the producers.  issue(i, s) queues the wgmmas of block i from stage s.
+template <typename Issue>
+__device__ __forceinline__ void mma_ring(int nkb, int stages, uint64_t *full, uint64_t *empty, bool leader, Issue issue) {
+    uint64_t *pending = nullptr;
+    for (int i = 0; i < nkb; ++i) {
+        const int s = i % stages;
+        mbar_wait(full + s, (i / stages) & 1);
+        wgmma_fence();
+        issue(i, s);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (pending && leader) mbar_arrive(pending);
+        pending = empty + s;
+    }
+    wgmma_wait<0>();
+    if (pending && leader) mbar_arrive(pending);
+}
+// ... and the hand-over: the ring is drained (every load was consumed), so the accumulator tile is laid over it.
+template <int BN>
+__device__ __forceinline__ void mma_publish(const AccTile<BN> &acc, float *tile, uint64_t *acc_full, int mt) {
+    mma_group_sync();
+    acc.store(tile, mt);
+    mma_group_sync();
+    if (mt == 0) mbar_arrive(acc_full);
+}
 
 
 // ---------------------------------------------------------------- host: tensor maps through the driver entry point
