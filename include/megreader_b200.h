@@ -131,6 +131,44 @@ int mr_db_loss_bwd_f32(const float *binary, const float *thresh, const float *th
                        const float *thresh_map, const float *thresh_mask, int N, int H, int W, float l1_scale, float bce_scale,
                        const void *workspace, const float *grad_out, float *d_binary, float *d_thresh, float *d_thresh_binary,
                        void *stream);
+/* Contour step of SegDetectorRepresenter (structure/representers/seg_detector_representer.py:60-80, csrc/db_boxes.cu):
+ *   contours = cv2.findContours(dest > thresh, RETR_LIST, CHAIN_APPROX_NONE)[:max_candidates]   per image, dest [N,1,H,W] fp32,
+ * thresh compared in fp32.  The contours are cv2's, array for array: same number, order and points (outer borders of the
+ * 8-connected foreground components and borders of the enclosed 4-connected background components, in descending raster order
+ * of their start pixels).  Outputs: count [N] = min(total, max_candidates), total [N] = number of contours in the image,
+ * offsets [N, max_candidates + 1] (contour c of image n is points[n, offsets[n][c] .. offsets[n][c + 1]); entries past count[n]
+ * hold the image's number of points), points [N, point_capacity, 2] (x, y) int32; points past point_capacity are not written
+ * (the offsets still count them).  workspace >= mr_db_contours_workspace_bytes(N, H, W, max_candidates).  MR_ERR_BAD_SHAPE for
+ * negative sizes, H * W >= 2^28 or a smaller workspace, before any CUDA call.  No host synchronisation. */
+int64_t mr_db_contours_workspace_bytes(int64_t N, int64_t H, int64_t W, int64_t max_candidates);
+int mr_db_contours_f32(const float *dest, int N, int H, int W, float thresh, int max_candidates, void *workspace,
+                       int64_t workspace_bytes, int *points, int64_t point_capacity, int *offsets, int *count, int *total,
+                       void *stream);
+/* The per-candidate steps before the unclip (seg_detector_representer.py:81-96) for every contour mr_db_contours_f32 kept,
+ * from its outputs: get_mini_boxes (:125-145: cv2.minAreaRect = convex hull + rotating calipers in float32 like cv2,
+ * cv2.boxPoints, the reference's corner order) and, where sside >= 3 (min_size), box_score_fast (:156-168: cv2.fillPoly of the box
+ * over its bounding rows / columns, cv2.mean of `binary` [N,1,H,W] under it, summed in double in raster order).
+ * boxes [N, max_candidates, 4, 2] (x, y) fp32, ssides [N, max_candidates] = min(width, height), scores [N, max_candidates] fp64
+ * (0 where sside < 3); entries c >= count[n] are zero, and a contour whose points did not fit point_capacity gets sside -1.
+ * The reference keeps a candidate when sside >= 3 and score >= box_thresh.  workspace >=
+ * mr_db_box_candidates_workspace_bytes(N, max_candidates, point_capacity). */
+int64_t mr_db_box_candidates_workspace_bytes(int64_t N, int64_t max_candidates, int64_t point_capacity);
+int mr_db_box_candidates_f32(const int *points, int64_t point_capacity, const int *offsets, const int *count, const float *binary,
+                             int N, int H, int W, int max_candidates, void *workspace, int64_t workspace_bytes, float *boxes,
+                             float *ssides, double *scores, void *stream);
+/* The whole of SegDetectorRepresenter.boxes_from_bitmap (seg_detector_representer.py:63-115) for a batch: the two entries above,
+ * then per candidate `box_thresh > score` (box_thresh compared in double), the unclip (GEOS ring area / length, Clipper 6.4.2
+ * round offset restated without its final union clean-up -- DESIGN §7), the second get_mini_boxes, sside >= 5, and the rescale
+ * clip(round(x / W * dest_w), 0, dest_w) in float32 with round-half-even; then the surviving boxes compacted in candidate order.
+ * binary, dest [N,1,H,W] fp32 (dest = the bitmap source: binary, thresh or thresh_binary); dest_sizes [N,2] int32 (h, w) on the
+ * device, or NULL for (H, W).  Outputs: boxes [N, max_candidates, 4, 2] int32 (x, y), scores [N, max_candidates] fp32, count [N];
+ * entries past count[n] are zero.  workspace >= mr_db_boxes_workspace_bytes(N, H, W, max_candidates): it holds find_contours'
+ * 4 * H * W points per image and 24 bytes of candidate scratch per point, i.e. about 136 bytes per pixel, plus the unclip
+ * scratch.  No host synchronisation: the call can be captured in a CUDA graph.  N <= 65535. */
+int64_t mr_db_boxes_workspace_bytes(int64_t N, int64_t H, int64_t W, int64_t max_candidates);
+int mr_db_boxes_f32(const float *binary, const float *dest, int N, int H, int W, float thresh, double box_thresh, int max_candidates,
+                    const int *dest_sizes, void *workspace, int64_t workspace_bytes, int *boxes, float *scores, int *count,
+                    void *stream);
 
 /* ------------------------------------------------------------------------------------------------
  * 1D CTC head of the CRNN decoder (replaces the `log_softmax -> nn.CTCLoss(zero_infinity=True)` call,
