@@ -357,6 +357,19 @@ int mr_conv2d_wgrad_tcgen05(const void *dz, const void *x, float *dWm, int N, in
 /* Implicit-GEMM weight gradient: dWm[Cout, kh*kw*C] fp32 += dz[N,Ho,Wo,Cout]^T (*) x[N,H,W,C] (atomic, split-K). */
 int mr_conv_wgrad_tcgen05(const void *dz, const void *x, float *dWm, int N, int H, int W, int C, int Cout, int kh, int kw,
                           int ph, int pw, int splits, void *stream);
+/* The CRNN backbone's convolutions on persistent ping-pong wgmma kernels (csrc/conv_pingpong.cu): stride 1, NHWC bf16 ->
+ * bf16, no bias or activation.  y[N*Ho*Wo, Cout] = conv(x[N,H,W,C], Wm[Cout, kh*kw*C]), bit-identical to
+ * mr_conv_fprop_tcgen05's bf16 output; with flipped/transposed weights and padding (k-1-p) the input gradient.
+ * MR_ERR_UNSUPPORTED unless C % 64 == 0, Cout % 8 == 0, 16-byte aligned pointers and an output that tiles with at most
+ * four TMA box segments (the caller then uses mr_conv_fprop_tcgen05). */
+int mr_conv_fprop_pp(const void *x, const void *Wm, void *y, int N, int H, int W, int C, int Cout, int kh, int kw, int ph,
+                     int pw, void *stream);
+/* Weight gradient of the same convolutions on a persistent wgmma kernel with 128 x 256 tiles (csrc/conv_pingpong.cu):
+ * dWm[Cout, kh*kw*C] fp32 += dz[N,Ho,Wo,Cout]^T (*) x[N,H,W,C], ACCUMULATED atomically (zero it first).  The K blocks of
+ * all tiles are split evenly over `ctas` CTAs (<= 0: one per SM).  MR_ERR_UNSUPPORTED unless C % 64 == 0, Cout % 8 == 0
+ * and 16-byte aligned pointers (the caller then uses mr_conv_wgrad_tcgen05). */
+int mr_conv_wgrad_pp(const void *dz, const void *x, float *dWm, int N, int H, int W, int C, int Cout, int kh, int kw, int ph,
+                     int pw, int ctas, void *stream);
 
 /* Fused LSTM time steps on wgmma (recurrent GEMM + cell in one launch, both directions): gate columns are
  * UNIT-MAJOR (column 4*j + g = gate g in {i,f,g,o} of hidden unit j), H % 64 == 0, bf16.  Every per-direction argument

@@ -27,8 +27,10 @@ USE_TCGEN05 = __import__("os").environ.get("MEGREADER_B200_TCGEN05", "1") != "0"
 LSTM_MODE = __import__("os").environ.get("MEGREADER_B200_LSTM", "seq")
 if __import__("os").environ.get("MEGREADER_B200_LSTM_FUSED", "0") == "1":     # older switch
     LSTM_MODE = "step"
-# conv weight gradients on a side stream, overlapped with the rest of the backward chain (MEGREADER_B200_WGRAD_STREAM=0: off)
-WGRAD_SIDE_STREAM = __import__("os").environ.get("MEGREADER_B200_WGRAD_STREAM", "1") == "1"
+# conv weight gradients on a side stream, overlapped with the rest of the backward chain (MEGREADER_B200_WGRAD_STREAM=1: on).
+# Off by default: the convolutions of the backward run on persistent kernels with one CTA per SM (185 to 230 KB of shared
+# memory each, csrc/conv_pingpong.cu), which leave no SM for a side stream to fill; see DESIGN.md section 4 for the step times.
+WGRAD_SIDE_STREAM = __import__("os").environ.get("MEGREADER_B200_WGRAD_STREAM", "0") == "1"
 _SIDE_STREAMS = {}
 
 
@@ -105,6 +107,20 @@ def _weight_grad(dWm, Cin, Cp, kh, kw):
     return dWm[:, :kh * kw * Cp].reshape(Cout, kh, kw, Cp)[..., :Cin].permute(0, 3, 1, 2).contiguous()
 
 
+def _conv_fprop(x, Wm, kh, kw, ph, pw):
+    """Stride-1 bf16 convolution (forward or input gradient) on the persistent ping-pong kernel; the one-tile-per-CTA
+    kernel only for geometries the former refuses.  Both give the same bits."""
+    r = ops.conv_fprop_pp(x, Wm, kh, kw, ph, pw)
+    return r if r is not None else ops.conv_fprop_tc(x, Wm, kh, kw, ph, pw)
+
+
+def _conv_wgrad(dz, x, kh, kw, ph, pw, out=None):
+    """Weight gradient [Cout, kh*kw*C] fp32 (accumulated into a zeroed `out` if given) on the persistent 128 x 256 kernel;
+    the one-tile-per-CTA kernel only for geometries the former refuses."""
+    r = ops.conv_wgrad_pp(dz, x, kh, kw, ph, pw, out=out)
+    return r if r is not None else ops.conv_wgrad_tc(dz, x, kh, kw, ph, pw, out=out)
+
+
 class _BackboneFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, module, bn_batch_stats, save, dtype, *params):
@@ -128,8 +144,8 @@ class _BackboneFn(torch.autograd.Function):
             Wm = _weight_matrix(conv.weight, C, Kp, dtype)
             implicit = USE_TCGEN05 and dtype == torch.bfloat16 and C % 64 == 0
             if implicit:
-                # wgmma implicit GEMM: activation tiles are gathered straight into swizzled smem, no im2col in HBM
-                z, Ho, Wo = ops.conv_fprop_tc(a, Wm, kh, kw, ph, pw)
+                # wgmma implicit GEMM: activation tiles come by TMA straight into swizzled smem, no im2col in HBM
+                z, Ho, Wo = _conv_fprop(a, Wm, kh, kw, ph, pw)
                 col = None
             else:
                 col, Ho, Wo = ops.im2col(a, kh, kw, ph, pw, Kp)
@@ -174,9 +190,10 @@ class _BackboneFn(torch.autograd.Function):
         dtype = ctx.dtype
         dy = ops.cast(dfeat.permute(0, 2, 3, 1).contiguous(), dtype).view(N * Hf * Wf, Cf)
         grads = []
-        # The weight gradients are off the critical path (dz_L -> dgrad_L -> pool/BN backward_{L-1} -> ...): they run on a
-        # side stream and fill the SMs that the HBM-bound elementwise kernels and the tail waves of the dgrad kernels
-        # leave idle.  Joined before the gradients are handed back (also inside CUDA-graph capture: fork/join by events).
+        # The weight gradients are off the critical path (dz_L -> dgrad_L -> pool/BN backward_{L-1} -> ...).  With
+        # WGRAD_SIDE_STREAM they run on a side stream, meant to fill SMs that the HBM-bound elementwise kernels leave idle,
+        # and are joined before the gradients are handed back (also inside CUDA-graph capture: fork/join by events);
+        # otherwise they run in order on the current stream.
         main = torch.cuda.current_stream(dfeat.device)
         side = _side_stream(dfeat.device) if WGRAD_SIDE_STREAM else None
         deferred = []                                   # (slot in grads, dWm, Cin, C, kh, kw) finished after the join
@@ -212,10 +229,10 @@ class _BackboneFn(torch.autograd.Function):
                     dz.record_stream(side)
                     rec["x"].record_stream(side)
                     with torch.cuda.stream(side):
-                        ops.conv_wgrad_tc(dz4, rec["x"], kh, kw, ph, pw, out=dWm)
+                        _conv_wgrad(dz4, rec["x"], kh, kw, ph, pw, dWm)
                     deferred.append((dWm, rec["Cin"], C, kh, kw))
                 else:
-                    dWm = ops.conv_wgrad_tc(dz4, rec["x"], kh, kw, ph, pw)                 # [Cout, K] fp32
+                    dWm = _conv_wgrad(dz4, rec["x"], kh, kw, ph, pw)                       # [Cout, K] fp32
                     dW = _weight_grad(dWm, rec["Cin"], C, kh, kw)
             else:
                 dWm = ops.gemm(dz, rec["col"], transA=True, out_dtype=torch.float32)      # [Cout, Kp]
@@ -230,7 +247,7 @@ class _BackboneFn(torch.autograd.Function):
                         Wd = ops.conv_weight_pack(wsrc, C, kh * kw * C, dtype, 1)          # flipped + transposed, one launch
                     else:
                         Wd = ops.cast(wsrc.flip(2, 3).permute(1, 2, 3, 0).reshape(C, kh * kw * Cout).contiguous(), dtype)
-                    dy, _, _ = ops.conv_fprop_tc(dz4, Wd, kh, kw, kh - 1 - ph, kw - 1 - pw)
+                    dy, _, _ = _conv_fprop(dz4, Wd, kh, kw, kh - 1 - ph, kw - 1 - pw)
                 else:
                     dcol = ops.gemm(dz, rec["Wm"])                                           # [P, Kp]
                     dy = ops.col2im(dcol, Nn, H, W, C, kh, kw, ph, pw).view(Nn * H * W, C)

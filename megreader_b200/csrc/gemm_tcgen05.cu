@@ -173,17 +173,12 @@ struct ConvArgs {
     const bf16 *x;
     int N, H, W, C, kh, kw, ph, pw, Ho, Wo;
     int sh, sw, dh, dw;                 // stride and dilation (round 2: ResNet trunks; 1 / 1 for the CRNN layers)
-    // TMA-A variant: the output space [N, Ho, Wo] is tiled by boxes of bw x bh x bn = 128 pixels; the width is cut
-    // into segments of power-of-two widths (e.g. Wo = 65 -> one 64-wide segment + one 1-wide segment).
-    struct Seg { int w0, bw, bh, bn, h_blocks, tile_begin; } seg[4];
+    // TMA-A variant: the output space [N, Ho, Wo] is tiled by the 128-pixel boxes of plan_conv_segments (wgmma.cuh).
+    ConvSeg seg[kMaxConvSegs];
     int nseg;
     GemmArgs g;        // M = N*Ho*Wo, N = Cout, K = kh*kw*C
 };
 
-__device__ __forceinline__ void tma_load_4d(const CUtensorMap *map, uint64_t *bar, void *dst, int c0, int c1, int c2, int c3) {
-    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
 __device__ __forceinline__ void cp_async16_zfill(uint32_t dst, const void *src, uint32_t src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
@@ -676,25 +671,6 @@ int launch(const CUtensorMap &ta, const CUtensorMap &tb, const GemmArgs &g, int 
                          "gemm_tcgen05 smem attr", "gemm_tcgen05_kernel", ta, tb, g);
 }
 
-// 4-D bf16 NHWC tensor map {C, W, H, N}, box {64, box_w, 1, 1}
-// sw / sh > 1: strided traversal (every sw-th column, sh-th row) -- the box then spans box_w * sw columns of the tensor and
-// delivers box_w of them (cuTensorMapEncodeTiled elementStrides)
-int make_map_nhwc(CUtensorMap *m, const void *base, int64_t C, int64_t W, int64_t H, int64_t N, int box_w, int box_h = 1,
-                  int box_n = 1, int sw = 1, int sh = 1) {
-    EncodeTiledFn fn = encode_fn();
-    if (!fn) { set_cuda_error(cudaErrorUnknown, "cuTensorMapEncodeTiled entry point"); return MR_ERR_CUDA; }
-    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-    cuuint32_t box[4] = {64, (cuuint32_t)(box_w * sw), (cuuint32_t)(box_h * sh), (cuuint32_t)box_n};
-    cuuint32_t estr[4] = {1, (cuuint32_t)sw, (cuuint32_t)sh, 1};
-    if (box[1] > 256 || box[2] > 256) { set_cuda_error(cudaErrorInvalidValue, "conv tensor map: strided box too large"); return MR_ERR_UNSUPPORTED; }
-    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_cuda_error(cudaErrorInvalidValue, "cuTensorMapEncodeTiled(4d)"); return MR_ERR_CUDA; }
-    return MR_OK;
-}
-
 template <int BN, int STAGES, int TMA_A>
 int launch_conv(const CUtensorMap &tb, const CUtensorMap *tx, const ConvArgs &a, int tiles, cudaStream_t st) {
     dim3 grid(TMA_A ? (unsigned)tiles : (unsigned)ceil_div(a.g.M, BM), (unsigned)ceil_div(a.g.N, BN), 1);
@@ -806,33 +782,12 @@ int mr_conv2d_fprop_tcgen05(const void *x, const void *Wm, void *y, int N, int H
     CUtensorMap tx[4];
     int tiles = 0;
     if (!no_tma_a) {
-        int w0 = 0;
-        bool ok = true;
-        while (ok && w0 < a.Wo) {                        /* ok = false: a box the TMA cannot take -> gather */
-            if (a.nseg == 4) { ok = false; break; }
-            int bw = 128;
-            while (bw > a.Wo - w0) bw >>= 1;
-            int nrep = (a.Wo - w0) / bw;                  /* consecutive segments of this width share geometry */
-            int bh = 1;
-            while (bh * 2 <= a.Ho && bw * bh * 2 <= 128) bh <<= 1;
-            const int bn = 128 / (bw * bh);
-            const int h_blocks = (int)ceil_div(a.Ho, bh), n_blocks = (int)ceil_div(N, bn);
-            for (int rep = 0; rep < nrep && ok; ++rep) {
-                if (a.nseg == 4) { ok = false; break; }
-                ConvArgs::Seg &sg = a.seg[a.nseg];
-                sg.w0 = w0; sg.bw = bw; sg.bh = bh; sg.bn = bn; sg.h_blocks = h_blocks; sg.tile_begin = tiles;
-                rc = make_map_nhwc(&tx[a.nseg], x, C, W, H, N, bw, bh, bn, sw, sh);
-                if (rc == MR_ERR_UNSUPPORTED) { ok = false; break; }
-                if (rc) return rc;
-                tiles += h_blocks * n_blocks;
-                ++a.nseg;
-                w0 += bw;
-            }
-        }
-        if (ok && a.nseg > 0) {
+        rc = plan_conv_segments(x, N, H, W, C, a.Ho, a.Wo, sh, sw, a.seg, tx, &a.nseg, &tiles);
+        if (rc) return rc;
+        if (a.nseg > 0) {
             for (int q = a.nseg; q < 4; ++q) tx[q] = tx[0];
-            /* shallow rings leave room for 2-3 CTAs per SM, so one CTA's epilogue overlaps another's main loop
-             * (the kernel is not persistent); MR_CONV_SHALLOW=0/1 overrides the default for experiments. */
+            /* The default shallow ring is not an occupancy choice: at 154 registers x 384 threads only one CTA fits on
+             * an SM whatever the ring depth.  MR_CONV_SHALLOW=0/1 overrides the default for experiments. */
             const char *sh_env = getenv("MR_CONV_SHALLOW");
             const bool shallow = sh_env ? sh_env[0] == '1' : true;
             if (shallow) {

@@ -1,8 +1,9 @@
 // Shared sm_90a building blocks: PTX wrappers for mbarrier / TMA / wgmma, the shared-memory matrix descriptors, the
 // operand ring of the one-shot kernels (layout, barriers, the MMA warpgroup's K loop), the accumulator hand-over from
 // the MMA warpgroup to the epilogue warps, and host-side tensor-map construction through the driver entry point (no
-// libcuda link dependency).  Included by gemm_tcgen05.cu, lstm_seq_tcgen05.cu and dcn_tcgen05.cu (the file names
-// predate the Hopper port; nothing in them is tcgen05 any more).
+// libcuda link dependency), and the 128-pixel box plan of the TMA convolutions.  Included by gemm_tcgen05.cu,
+// lstm_seq_tcgen05.cu, dcn_tcgen05.cu (the file names predate the Hopper port; nothing in them is tcgen05 any more) and
+// conv_pingpong.cu.
 #pragma once
 #include "common.cuh"
 #include <cuda.h>
@@ -43,6 +44,35 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap *map, uint64_t *bar, void *dst, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void tma_load_4d(const CUtensorMap *map, uint64_t *bar, void *dst, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+// shared -> global tensor store; completion is tracked per thread by bulk groups (commit, then wait)
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap *map, const void *src, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                 ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the stores committed before the last N groups have finished reading shared memory (their source may be overwritten)
+template <int N> __device__ __forceinline__ void bulk_wait_group_read() {
+    asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// ... and have finished writing global memory
+template <int N> __device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// four 8x8 b16 matrices to shared memory: register i of every lane is matrix i's fragment in the mma accumulator layout
+// (lane l holds row l / 4, columns 2 (l % 4), +1); lanes 8i..8i+7 give the addresses of matrix i's eight 16-byte rows
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+                 "r"(r3) : "memory");
+}
+// named barriers: `count` threads (whole warps) of the CTA; arrive does not wait
+template <int COUNT> __device__ __forceinline__ void named_bar_sync(int id) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "n"(COUNT) : "memory");
+}
+template <int COUNT> __device__ __forceinline__ void named_bar_arrive(int id) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "n"(COUNT) : "memory");
 }
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap *map) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
@@ -313,6 +343,63 @@ int make_map(CUtensorMap *m, const void *base, int64_t inner, int64_t outer, int
                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_cuda_error(cudaErrorInvalidValue, "cuTensorMapEncodeTiled"); return MR_ERR_CUDA; }
+    return MR_OK;
+}
+
+// 4-D bf16 NHWC tensor map {C, W, H, N}, box {64, box_w, box_h, box_n}
+// sw / sh > 1: strided traversal (every sw-th column, sh-th row) -- the box then spans box_w * sw columns of the tensor and
+// delivers box_w of them (cuTensorMapEncodeTiled elementStrides)
+int make_map_nhwc(CUtensorMap *m, const void *base, int64_t C, int64_t W, int64_t H, int64_t N, int box_w, int box_h = 1,
+                  int box_n = 1, int sw = 1, int sh = 1) {
+    EncodeTiledFn fn = encode_fn();
+    if (!fn) { set_cuda_error(cudaErrorUnknown, "cuTensorMapEncodeTiled entry point"); return MR_ERR_CUDA; }
+    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+    cuuint32_t box[4] = {64, (cuuint32_t)(box_w * sw), (cuuint32_t)(box_h * sh), (cuuint32_t)box_n};
+    cuuint32_t estr[4] = {1, (cuuint32_t)sw, (cuuint32_t)sh, 1};
+    if (box[1] > 256 || box[2] > 256) { set_cuda_error(cudaErrorInvalidValue, "conv tensor map: strided box too large"); return MR_ERR_UNSUPPORTED; }
+    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(base), dims, strides, box, estr,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_cuda_error(cudaErrorInvalidValue, "cuTensorMapEncodeTiled(4d)"); return MR_ERR_CUDA; }
+    return MR_OK;
+}
+
+// ---------------------------------------------------------------- 128-pixel output tiles of the TMA convolutions
+// The output space [N, Ho, Wo] is tiled by boxes of bw x bh x bn = 128 pixels; the width is cut into segments of
+// power-of-two widths (e.g. Wo = 65 -> one 64-wide segment + one 1-wide segment), each with its own activation tensor map.
+// Tile row r of a box is pixel (n0 + r / (bw bh), h0 + r / bw % bh, w0 + r % bw): the row order of the TMA box itself.
+constexpr int kMaxConvSegs = 4;
+struct ConvSeg { int w0, bw, bh, bn, h_blocks, tile_begin; };
+
+// Plans the segments of an [N, Ho, Wo] output over the activation x [N, H, W, C] (stride sw, sh) and encodes one tensor map
+// per segment into tx.  *nseg = 0 when the plan needs more than kMaxConvSegs segments or a box the TMA cannot take;
+// *tiles = the number of 128-pixel tiles of all segments.
+int plan_conv_segments(const void *x, int N, int H, int W, int C, int Ho, int Wo, int sh, int sw, ConvSeg *seg,
+                       CUtensorMap *tx, int *nseg, int *tiles) {
+    *nseg = 0;
+    *tiles = 0;
+    int w0 = 0;
+    while (w0 < Wo) {
+        int bw = 128;
+        while (bw > Wo - w0) bw >>= 1;
+        const int nrep = (Wo - w0) / bw;                  /* consecutive segments of this width share geometry */
+        int bh = 1;
+        while (bh * 2 <= Ho && bw * bh * 2 <= 128) bh <<= 1;
+        const int bn = 128 / (bw * bh);
+        const int h_blocks = (int)ceil_div(Ho, bh), n_blocks = (int)ceil_div(N, bn);
+        for (int rep = 0; rep < nrep; ++rep) {
+            if (*nseg == kMaxConvSegs) { *nseg = 0; return MR_OK; }
+            ConvSeg &sg = seg[*nseg];
+            sg.w0 = w0; sg.bw = bw; sg.bh = bh; sg.bn = bn; sg.h_blocks = h_blocks; sg.tile_begin = *tiles;
+            const int rc = make_map_nhwc(&tx[*nseg], x, C, W, H, N, bw, bh, bn, sw, sh);
+            if (rc == MR_ERR_UNSUPPORTED) { *nseg = 0; return MR_OK; }
+            if (rc) return rc;
+            *tiles += h_blocks * n_blocks;
+            ++*nseg;
+            w0 += bw;
+        }
+    }
     return MR_OK;
 }
 
