@@ -170,6 +170,24 @@ int mr_db_boxes_f32(const float *binary, const float *dest, int N, int H, int W,
                     const int *dest_sizes, void *workspace, int64_t workspace_bytes, int *boxes, float *scores, int *count,
                     void *stream);
 
+/* Training targets of the DB detector (data/processes/make_seg_detection_data.py:21-100, make_border_map.py:24-121,
+ * csrc/db_targets.cu) for a batch of N images of H x W after RandomCropData.  polygons [capacity, 4, 2] (dtype 0 = float32,
+ * 1 = float64) hold the quads of image n at rows offsets[n] .. offsets[n + 1] (device int32 [N + 1], non-decreasing, at most
+ * capacity; rows past offsets[N] are unused), ignore_tags [capacity] uint8.  shrink_k = 1 - shrink_ratio^2 (double, as numpy
+ * computes it), min_text_size, thresh_scale = float32(thresh_max - thresh_min), thresh_min.  Writes gt [N,1,H,W], mask,
+ * thresh_map and thresh_mask [N,H,W] (float32), polygons_out (validate_polygons' clipped and reordered quads, same dtype),
+ * ignore_out (the updated tags) and status [capacity] (int32 bits: 1 ignored on input, 2 |area| < 1, 4 side < min_text_size,
+ * 8 shrink empty, 16 shrink in several pieces (largest used), 32 pad empty (no border map), 64 pad in several pieces
+ * (largest used), 128 clean-up scratch too small (treated as empty)).  workspace >= mr_db_targets_workspace_bytes(N, H, W,
+ * capacity): about 120 KB per polygon slot at 640 x 640.  MR_ERR_BAD_SHAPE for N outside 1..65535, H * W >= 2^28, sides above
+ * 65535, a bad dtype or a smaller workspace, before any CUDA call.  No host synchronisation: the call can be captured in a CUDA
+ * graph and replayed with new polygon contents. */
+int64_t mr_db_targets_workspace_bytes(int64_t N, int64_t H, int64_t W, int64_t capacity);
+int mr_db_targets(const void *polygons, int dtype, const unsigned char *ignore_tags, const int *offsets, int N, int H, int W,
+                  int capacity, double shrink_k, double min_text_size, float thresh_scale, float thresh_min, void *workspace,
+                  int64_t workspace_bytes, float *gt, float *mask, float *thresh_map, float *thresh_mask, void *polygons_out,
+                  unsigned char *ignore_out, int *status, void *stream);
+
 /* ------------------------------------------------------------------------------------------------
  * 1D CTC head of the CRNN decoder (replaces the `log_softmax -> nn.CTCLoss(zero_infinity=True)` call,
  * decoders/crnn.py:47-48,95-99; arithmetic restated in decoders/ctc_loss.py:65-122).  fp32.

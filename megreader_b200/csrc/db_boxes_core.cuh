@@ -518,59 +518,73 @@ __host__ __device__ inline bool clip_line(int64_t width, int64_t height, L2 &p1,
     return (c1 | c2) == 0;
 }
 
+// One edge of cv::CollectPolyEdges (LINE_8, shift 0) from (x0, y0) to (x1, y1) on a width x height image: the ends of the
+// 8-connected line cv2 draws for it, clipped to the image (*draw false when nothing of it is inside), and its PolyEdge of the
+// scan-line fill in 16.16 fixed point (false for a horizontal edge, which has none).  An edge with an end outside the image
+// takes the clipped ends' x (and their y unless the clipped segment is horizontal).
+struct PolyEdge { int y0, y1; int64_t x, dx; int next; };
+
+__host__ __device__ inline bool poly_edge(int x0, int y0, int x1, int y1, int width, int height, L2 &a, L2 &b, bool &draw,
+                                          PolyEdge &ed) {
+    const int XY_SHIFT = 16;
+    const L2 pt0{(int64_t)x0 << XY_SHIFT, y0}, pt1{(int64_t)x1 << XY_SHIFT, y1};
+    a = L2{x0, y0};
+    b = L2{x1, y1};
+    const bool outside = (uint64_t)a.x >= (uint64_t)width || (uint64_t)b.x >= (uint64_t)width ||
+                         (uint64_t)a.y >= (uint64_t)height || (uint64_t)b.y >= (uint64_t)height;
+    draw = !outside || clip_line(width, height, a, b);
+    L2 c0 = pt0, c1 = pt1;
+    if (outside) {
+        if (a.y != b.y) { c0.y = a.y; c1.y = b.y; }
+        c0.x = a.x << XY_SHIFT;
+        c1.x = b.x << XY_SHIFT;
+    }
+    if (pt0.y == pt1.y) return false;
+    ed.dx = (c1.x - c0.x) / (c1.y - c0.y);
+    if (pt0.y < pt1.y) {
+        ed.y0 = (int)pt0.y; ed.y1 = (int)pt1.y;
+        ed.x = c0.x + (ed.y0 - c0.y) * ed.dx;
+    } else {
+        ed.y0 = (int)pt1.y; ed.y1 = (int)pt0.y;
+        ed.x = c1.x + (ed.y0 - c1.y) * ed.dx;
+    }
+    return true;
+}
+
+// Line(img, a, b): cv::LineIterator(.., 8, leftToRight = true) over the clipped ends; visit(x, y) per pixel
+template <class Visit>
+__host__ __device__ inline void draw_line(L2 u, L2 v, Visit visit) {
+    int64_t sy = 1, dx = v.x - u.x, dy = v.y - u.y;
+    if (dx < 0) { dx = -dx; dy = -dy; const L2 t = u; u = v; v = t; }
+    if (dy < 0) { dy = -dy; sy = -1; }
+    const bool vert = dy > dx;
+    if (vert) { const int64_t t = dx; dx = dy; dy = t; }
+    int64_t err = dx - (dy + dy), x = u.x, y = u.y;
+    for (int64_t k = 0; k <= dx; ++k) {
+        visit((int)x, (int)y);
+        const bool m = err < 0;
+        err += -(dy + dy) + (m ? dx + dx : 0);
+        if (vert) { y += sy; if (m) x += 1; }
+        else { x += 1; if (m) y += sy; }
+    }
+}
+
 // The pixels cv2.fillPoly(mask, [quad], 1) sets on a width x height mask (LINE_8, shift 0): the four edges drawn as
-// 8-connected lines (cv::LineIterator, left to right, clipped to the mask), and the scan-line fill of the edge collection in
-// 16.16 fixed point (from the ceiling of the left edge to the floor of the right one, clipped to the mask).  visit(x, y) is
-// called for every set pixel, possibly more than once; the scan-line fill stops before row y_stop (rows above it do not
-// depend on the rows below).
+// 8-connected lines (clipped to the mask), and the scan-line fill of the edge collection in 16.16 fixed point (from the
+// ceiling of the left edge to the floor of the right one, clipped to the mask).  visit(x, y) is called for every set pixel,
+// possibly more than once; the scan-line fill stops before row y_stop (rows above it do not depend on the rows below).
 template <class Visit>
 __host__ __device__ inline void fill_quad(const int *q, int width, int height, int y_stop, Visit visit) {
     const int XY_SHIFT = 16;
     const int64_t XY_ONE = (int64_t)1 << XY_SHIFT;
-    struct Edge { int y0, y1; int64_t x, dx; int next; };
-    Edge all[6];
+    PolyEdge all[6];
     int ne = 0;
-    L2 pt0{(int64_t)q[6] << XY_SHIFT, q[7]};
     for (int i = 0; i < 4; ++i) {
-        const L2 pt1{(int64_t)q[2 * i] << XY_SHIFT, q[2 * i + 1]};
-        const L2 t0{(pt0.x + (XY_ONE >> 1)) >> XY_SHIFT, pt0.y}, t1{(pt1.x + (XY_ONE >> 1)) >> XY_SHIFT, pt1.y};
-        const bool outside = (uint64_t)t0.x >= (uint64_t)width || (uint64_t)t1.x >= (uint64_t)width ||
-                             (uint64_t)t0.y >= (uint64_t)height || (uint64_t)t1.y >= (uint64_t)height;
-        L2 a = t0, b = t1;
-        if (!outside || clip_line(width, height, a, b)) {      // Line(img, t0, t1): LineIterator(.., 8, leftToRight = true)
-            L2 u = a, v = b;
-            int64_t sy = 1, dx = v.x - u.x, dy = v.y - u.y;
-            if (dx < 0) { dx = -dx; dy = -dy; const L2 t = u; u = v; v = t; }
-            if (dy < 0) { dy = -dy; sy = -1; }
-            const bool vert = dy > dx;
-            if (vert) { const int64_t t = dx; dx = dy; dy = t; }
-            int64_t err = dx - (dy + dy), x = u.x, y = u.y;
-            for (int64_t k = 0; k <= dx; ++k) {
-                visit((int)x, (int)y);
-                const bool m = err < 0;
-                err += -(dy + dy) + (m ? dx + dx : 0);
-                if (vert) { y += sy; if (m) x += 1; }
-                else { x += 1; if (m) y += sy; }
-            }
-        }
-        L2 c0 = pt0, c1 = pt1;                   // an edge with an end outside the mask takes the clipped ends' x (and their
-        if (outside) {                           // y unless the clipped segment is horizontal)
-            if (a.y != b.y) { c0.y = a.y; c1.y = b.y; }
-            c0.x = a.x << XY_SHIFT;
-            c1.x = b.x << XY_SHIFT;
-        }
-        if (pt0.y != pt1.y) {
-            Edge &ed = all[ne++];
-            ed.dx = (c1.x - c0.x) / (c1.y - c0.y);
-            if (pt0.y < pt1.y) {
-                ed.y0 = (int)pt0.y; ed.y1 = (int)pt1.y;
-                ed.x = c0.x + (ed.y0 - c0.y) * ed.dx;
-            } else {
-                ed.y0 = (int)pt1.y; ed.y1 = (int)pt0.y;
-                ed.x = c1.x + (ed.y0 - c1.y) * ed.dx;
-            }
-        }
-        pt0 = pt1;
+        const int k = (i + 3) & 3;
+        L2 a, b;
+        bool draw;
+        if (poly_edge(q[2 * k], q[2 * k + 1], q[2 * i], q[2 * i + 1], width, height, a, b, draw, all[ne])) ++ne;
+        if (draw) draw_line(a, b, visit);
     }
     // FillEdgeCollection
     if (ne < 2) return;
@@ -588,9 +602,9 @@ __host__ __device__ inline void fill_quad(const int *q, int width, int height, i
     if (y_max < 0 || y_min >= height || x_max < 0 || x_min >= ((int64_t)width << XY_SHIFT)) return;
     for (int i = 1; i < ne; ++i)                 // std::sort of <= 4 edges (an insertion sort) by (y0, x, dx)
         for (int j = i; j > 0; --j) {
-            const Edge &p = all[j - 1], &c = all[j];
+            const PolyEdge &p = all[j - 1], &c = all[j];
             if (!(c.y0 != p.y0 ? c.y0 < p.y0 : c.x != p.x ? c.x < p.x : c.dx < p.dx)) break;
-            const Edge t = all[j]; all[j] = all[j - 1]; all[j - 1] = t;
+            const PolyEdge t = all[j]; all[j] = all[j - 1]; all[j - 1] = t;
         }
     const int TMP = 5;                           // the list head; edge `ne` is the y0 = INT_MAX sentinel
     all[ne].y0 = INT32_MAX;
@@ -721,8 +735,9 @@ __host__ __device__ inline double box_score(const float *pred, int H, int W, con
 // can differ.  This restatement is not pinned against pyclipper (not a dependency of the project); tests pin its invariants. ----
 namespace mr_dbbox {
 
-// GEOS Area::ofRing and Length::ofLine of the closed ring box[0..3], box[0]
-__host__ __device__ inline double unclip_distance(const float *box) {
+// GEOS Area::ofRing and Length::ofLine of the closed ring box[0..3], box[0] (float or double corners)
+template <class T>
+__host__ __device__ inline void ring_area_length(const T *box, double &area, double &length) {
     double x[5], y[5];
     for (int i = 0; i < 5; ++i) { x[i] = box[2 * (i & 3)]; y[i] = box[2 * (i & 3) + 1]; }
     double sum = 0., len = 0.;
@@ -731,15 +746,23 @@ __host__ __device__ inline double unclip_distance(const float *box) {
         const double dx = dsub(x[i + 1], x[i]), dy = dsub(y[i + 1], y[i]);
         len = dadd(len, sqrt(dadd(dmul(dx, dx), dmul(dy, dy))));
     }
-    const double area = fabs(sum / 2.);
+    area = fabs(sum / 2.);
+    length = len;
+}
+
+__host__ __device__ inline double unclip_distance(const float *box) {
+    double area, len;
+    ring_area_length(box, area, len);
     return dmul(area, 1.5) / len;
 }
 
 __host__ __device__ inline int64_t clipper_round(double v) { return v < 0 ? (int64_t)dsub(v, 0.5) : (int64_t)dadd(v, 0.5); }
 
-// The offset path of the box (int points into ox / oy, at most cap of them).  Returns the number of points, 0 when the
-// truncated box has fewer than three distinct points (Clipper then has no path), -1 when cap is too small.
-__host__ __device__ inline int unclip_offset(const float *box, double delta, int *ox, int *oy, int cap) {
+// The raw offset path of the box (float or double corners; delta > 0 pads, delta < 0 shrinks) before Execute's clean-up:
+// int points into ox / oy, at most cap of them.  Returns the number of points, 0 when the truncated box has fewer than three
+// distinct points (Clipper then has no path), -1 when cap is too small.
+template <class T>
+__host__ __device__ inline int unclip_offset(const T *box, double delta, int *ox, int *oy, int cap) {
     // AddPath: truncation to cInt, trailing copies of the first point and consecutive duplicates dropped
     int64_t px[4], py[4];
     int hi = 3;
