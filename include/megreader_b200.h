@@ -188,6 +188,25 @@ int mr_db_targets(const void *polygons, int dtype, const unsigned char *ignore_t
                   int64_t workspace_bytes, float *gt, float *mask, float *thresh_map, float *thresh_mask, void *polygons_out,
                   unsigned char *ignore_out, int *status, void *stream);
 
+/* Validation measure of the DB detector: QuadMeasurer.measure / DetectionIoUEvaluator.evaluate_image
+ * (concern/icdar2015_eval/detection/iou.py:13-179, csrc/db_measure.cu) for a batch of N images.  gt_polygons [capacity, 4, 2]
+ * (gt_dtype 0 = float32, 1 = float64) hold the gt quads of image n at rows offsets[n] .. offsets[n + 1] (device int32 [N + 1]);
+ * rows before offsets[0] or from offsets[N] on belong to no image.  ignore_tags [capacity] uint8; boxes [N, max_dets, 4, 2] (det_dtype 0 = int32, 1 = float64) hold count[n] (device int32 [N])
+ * detections of image n.  Outputs: gt_index / gt_match [capacity] (index among the image's valid gt, matched det's valid index;
+ * -1 for none), det_index / det_match [N, max_dets] (valid index, matched gt's valid index), det_dontcare [N, max_dets] uint8,
+ * image_counts [N, 5] int32 (care gt, care det, matched, valid gt, valid det), image_metrics [N, 3] float64 (precision,
+ * recall, hmean), image_status [N] int32 (1: offsets[n], offsets[n + 1] not non-decreasing within [0, capacity]; 2: count[n]
+ * outside [0, max_dets]; such an image adds nothing to totals), optional iou [capacity, max_dets] float64 (0 outside valid
+ * pairs of one image) and totals [3] int64, added into (care gt, care det, matched).  workspace >=
+ * mr_db_measure_workspace_bytes(N, capacity, max_dets).  MR_ERR_BAD_SHAPE for N < 1, capacity > 2^24, max_dets > 2^20, a bad
+ * dtype or a smaller workspace, before any CUDA call.  No host synchronisation: the call can be captured in a CUDA graph. */
+int64_t mr_db_measure_workspace_bytes(int64_t N, int64_t capacity, int64_t max_dets);
+int mr_db_measure(const void *gt_polygons, int gt_dtype, const unsigned char *ignore_tags, const int *offsets, int N, int capacity,
+                  const void *boxes, int det_dtype, const int *count, int max_dets, double iou_constraint,
+                  double area_precision_constraint, void *workspace, int64_t workspace_bytes, int *gt_index, int *gt_match,
+                  int *det_index, unsigned char *det_dontcare, int *det_match, int *image_counts, double *image_metrics,
+                  int *image_status, double *iou, long long *totals, void *stream);
+
 /* ------------------------------------------------------------------------------------------------
  * 1D CTC head of the CRNN decoder (replaces the `log_softmax -> nn.CTCLoss(zero_infinity=True)` call,
  * decoders/crnn.py:47-48,95-99; arithmetic restated in decoders/ctc_loss.py:65-122).  fp32.
