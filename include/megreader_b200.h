@@ -200,6 +200,31 @@ int mr_db_targets(const void *polygons, int dtype, const unsigned char *ignore_t
  * pairs of one image) and totals [3] int64, added into (care gt, care det, matched).  workspace >=
  * mr_db_measure_workspace_bytes(N, capacity, max_dets).  MR_ERR_BAD_SHAPE for N < 1, capacity > 2^24, max_dets > 2^20, a bad
  * dtype or a smaller workspace, before any CUDA call.  No host synchronisation: the call can be captured in a CUDA graph. */
+/* The DB detector's input batch (seg_detector_db.yaml: AugmentDetectionData, RandomCropData, MakeICDARData, NormalizeImage;
+ * csrc/db_batch.cu) for N images.  images: one buffer of HWC pixels (image_dtype 0 = uint8, 1 = float32; image_elems
+ * elements), image n at element image_offsets[n] (device int64 [N]) with shapes[n] = (h, w) (device int32 [N, 2]), each at
+ * most max_h x max_w.  polygons [capacity, 4, 2] (poly_dtype 0 = float32, 1 = float64), ignore_tags [capacity] uint8 and
+ * offsets [N + 1] int32 as mr_db_targets takes them.  mode 0 (training): draws [N, n_draws] float32 with n_draws >= 3 + 8 *
+ * max_tries (flip, angle, scale, then crop_area's picks), Fliplr(flip_p), Affine(rotate=(rotate_lo, rotate_hi)),
+ * Resize((scale_lo, scale_hi)) with scale_hi <= 4, RandomCropData(size = (out_w, out_h), max_tries, min_crop_side_ratio);
+ * mode 1 (validation): Resize to out_h x out_w, draws unused.  NormalizeImage subtracts (mean0, mean1, mean2).
+ * Outputs: image_out [N, 3, out_h, out_w] float32; polygons_out [capacity, 4, 2] float64, ignore_out [capacity] and
+ * offsets_out [N + 1]: the kept quads on the canvas compacted in input order, zero rows after; shape_out [N, 2] (the input's
+ * h, w), crop_out [N, 4] (x, y, w, h in the resized image), scale_out [N] float64, status [N] (bits: 1 shape outside 1..max or
+ * resized side beyond the workspace, 2 pixels outside the buffer, 4 offsets not non-decreasing within 0..capacity; such an
+ * image gets no quads and a zero canvas).  workspace >= mr_db_batch_workspace_bytes(N, max_h, max_w, capacity): about
+ * 12 bytes per pixel of N x max_h x max_w.  MR_ERR_BAD_SHAPE for N outside 1..65535, sides above 16384, bad modes, dtypes,
+ * draws or ranges, or a smaller workspace, before any CUDA call.  No host synchronisation: the call can be captured in a CUDA
+ * graph and replayed with new images, quads and draws. */
+int64_t mr_db_batch_workspace_bytes(int64_t N, int64_t max_h, int64_t max_w, int64_t capacity);
+int mr_db_batch(const void *images, int image_dtype, int64_t image_elems, const int64_t *image_offsets, const int *shapes, int N,
+                int max_h, int max_w, const void *polygons, int poly_dtype, const unsigned char *ignore_tags, const int *offsets,
+                int capacity, const float *draws, int n_draws, int mode, int out_h, int out_w, int max_tries,
+                double min_crop_side_ratio, double flip_p, double rotate_lo, double rotate_hi, double scale_lo, double scale_hi,
+                double mean0, double mean1, double mean2, void *workspace, int64_t workspace_bytes, float *image_out,
+                double *polygons_out, unsigned char *ignore_out, int *offsets_out, int *shape_out, int *crop_out, double *scale_out,
+                int *status, void *stream);
+
 int64_t mr_db_measure_workspace_bytes(int64_t N, int64_t capacity, int64_t max_dets);
 int mr_db_measure(const void *gt_polygons, int gt_dtype, const unsigned char *ignore_tags, const int *offsets, int N, int capacity,
                   const void *boxes, int det_dtype, const int *count, int max_dets, double iou_constraint,

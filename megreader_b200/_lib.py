@@ -107,6 +107,9 @@ _SIGS = {
     "mr_db_targets_workspace_bytes": [c_i64] * 4,
     "mr_db_targets": [c_p, c_int, c_p, c_p, c_int, c_int, c_int, c_int, ctypes.c_double, ctypes.c_double, c_f32, c_f32, c_p, c_i64]
                      + [c_p] * 8,
+    "mr_db_batch_workspace_bytes": [c_i64] * 4,
+    "mr_db_batch": [c_p, c_int, c_i64, c_p, c_p, c_int, c_int, c_int, c_p, c_int, c_p, c_p, c_int, c_p, c_int, c_int, c_int, c_int,
+                    c_int] + [ctypes.c_double] * 9 + [c_p, c_i64] + [c_p] * 9,
     "mr_db_measure_workspace_bytes": [c_i64] * 3,
     "mr_db_measure": [c_p, c_int, c_p, c_p, c_int, c_int, c_p, c_int, c_p, c_int, ctypes.c_double, ctypes.c_double, c_p, c_i64]
                      + [c_p] * 11,
@@ -117,6 +120,7 @@ _RESTYPES = {
     "mr_db_boxes_workspace_bytes": c_i64,
     "mr_db_targets_workspace_bytes": c_i64,
     "mr_db_measure_workspace_bytes": c_i64,
+    "mr_db_batch_workspace_bytes": c_i64,
     "mr_db_loss_workspace_bytes": c_i64,
     "mr_dcn_fused_workspace_bytes_h": c_i64,
     "mr_dcn_fused_backward_workspace_bytes_h": c_i64,

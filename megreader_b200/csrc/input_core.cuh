@@ -19,10 +19,19 @@ namespace mr_input {
 
 struct Axis { int i0, i1; float w0, w1; };
 
+// (d + 0.5) * scale - 0.5 in double with both roundings, as cv2's x86 build computes it (no fused multiply-add on the device)
+__host__ __device__ inline double src_coord(int d, double scale) {
+#ifdef __CUDA_ARCH__
+    return __dsub_rn(__dmul_rn((double)d + 0.5, scale), 0.5);
+#else
+    return ((double)d + 0.5) * scale - 0.5;
+#endif
+}
+
 // source taps of destination index d along an axis of `src` samples resized to `dst` samples
 __host__ __device__ inline Axis axis_taps(int d, int dst, int src, bool zero_fraction_at_border) {
     const double scale = 1.0 / ((double)dst / (double)src);
-    float f = (float)(((double)d + 0.5) * scale - 0.5);
+    float f = (float)src_coord(d, scale);
     int s = (int)floorf(f);
     f -= (float)s;
     Axis a;
@@ -44,6 +53,12 @@ template <typename S> __host__ __device__ inline float src_value(const S *img, i
     return (float)img[((int64_t)y * W + x) * 3 + c];
 }
 
+// NormalizeImage of one value: float32 array minus float64 vector, stored as float32, then / 255
+__host__ __device__ inline float normalize_value(float v, double mean_c) {
+    const float centred = (float)((double)v - mean_c);
+    return centred / 255.f;
+}
+
 // one output value: destination pixel (y, x), channel c of an image resized to [dst_h, valid_w] and placed at the left of a
 // [dst_h, dst_w] canvas (columns >= valid_w are the zero padding of mode "pad"), then normalised
 template <typename S>
@@ -56,8 +71,7 @@ __host__ __device__ inline float resize_normalize_value(const S *img, int H, int
         const float r1 = src_value(img, W, ay.i1, ax.i0, c) * ax.w0 + src_value(img, W, ay.i1, ax.i1, c) * ax.w1;
         v = r0 * ay.w0 + r1 * ay.w1;
     }
-    const float centred = (float)((double)v - mean_c);      // float32 array minus float64 vector, stored as float32
-    return centred / 255.f;
+    return normalize_value(v, mean_c);
 }
 
 // flat output index of [N, 3, dst_h, dst_w] -> (n, c, y, x)
