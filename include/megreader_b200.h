@@ -232,6 +232,35 @@ int mr_db_measure(const void *gt_polygons, int gt_dtype, const unsigned char *ig
                   int *det_index, unsigned char *det_dontcare, int *det_match, int *image_counts, double *image_metrics,
                   int *image_status, double *iou, long long *totals, void *stream);
 
+/* The text recognisers' validation measure (SequenceRecognitionMeasurer; csrc/rec_measure.cu) for a batch of N samples.
+ * Lexicon: n_words unique words as code points cp [offsets[n_words]] int32 with offsets [n_words + 1] int32 (device);
+ * mr_rec_lexicon_build fills `table` (>= mr_rec_lexicon_build_bytes(n_words) bytes: the words' hashes, then an open-addressing
+ * table of at least 2 x n_words slots, a power of two) and keeps no pointer to the words, which the measure reads again.
+ * Measure, label form (fold_len != NULL): gt [N, gt_width] and pred [N, pred_width] class ids (dtype 0 = int32, 1 = int64);
+ * fold_len [C] int32 and fold_cp [C, 4] int32 map each class to the code points of charset[id].upper() (none for blank and
+ * unknown); gt_len and pred_len are unused.  String form (fold_len == NULL): gt and pred are int32 code points already folded,
+ * with lengths gt_len [N] and pred_len [N].  The shorter width (times 4 in the label form) must not exceed 2048
+ * (MR_ERR_UNSUPPORTED).  Outputs per sample: accuracy (uint8: folded strings equal), distance (Levenshtein, int32),
+ * edit_distance (1 - min(L, d) / L, 0.0 for an empty gt, float64), in_lexicon (uint8: the folded gt is a word; 0 without a
+ * lexicon), the folded lengths and status (MR_REC_BAD_LABEL: an id outside [0, C); MR_REC_BAD_LENGTH: a length outside
+ * [0, width]).  totals, optional, MR_REC_TOTALS float64: six AverageMeters of gather_measure as (val, sum, count, updates)
+ * (accuracy, edit distance, in-lexicon accuracy, out-of-lexicon accuracy, in-lexicon edit distance, out-of-lexicon edit
+ * distance; the last four only with a lexicon), then the number of refused batches: a batch with any nonzero status updates
+ * no meter.  workspace >= mr_rec_measure_workspace_bytes(N, gt_width, pred_width, fold_len != NULL).  MR_ERR_BAD_SHAPE for
+ * N outside 1..2^24, widths above 2^20, bad dtypes or a smaller workspace, before any CUDA call.  No host synchronisation:
+ * the call can be captured in a CUDA graph. */
+#define MR_REC_BAD_LABEL 1
+#define MR_REC_BAD_LENGTH 2
+#define MR_REC_TOTALS 25
+int64_t mr_rec_lexicon_build_bytes(int64_t n_words);
+int mr_rec_lexicon_build(const int *cp, const int *offsets, int n_words, void *table, int64_t table_bytes, void *stream);
+int64_t mr_rec_measure_workspace_bytes(int64_t N, int64_t gt_width, int64_t pred_width, int folded);
+int mr_rec_measure(const void *gt, int gt_dtype, const int *gt_len, int gt_width, const void *pred, int pred_dtype, const int *pred_len,
+                   int pred_width, int N, const int *fold_len, const int *fold_cp, int C, const int *lex_cp, const int *lex_offsets,
+                   int n_words, const void *lex_table, void *workspace, int64_t workspace_bytes, unsigned char *accuracy,
+                   int *distance, double *edit_distance, unsigned char *in_lexicon, int *gt_folded_len, int *pred_folded_len,
+                   int *status, double *totals, void *stream);
+
 /* ------------------------------------------------------------------------------------------------
  * 1D CTC head of the CRNN decoder (replaces the `log_softmax -> nn.CTCLoss(zero_infinity=True)` call,
  * decoders/crnn.py:47-48,95-99; arithmetic restated in decoders/ctc_loss.py:65-122).  fp32.

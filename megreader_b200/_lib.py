@@ -113,6 +113,11 @@ _SIGS = {
     "mr_db_measure_workspace_bytes": [c_i64] * 3,
     "mr_db_measure": [c_p, c_int, c_p, c_p, c_int, c_int, c_p, c_int, c_p, c_int, ctypes.c_double, ctypes.c_double, c_p, c_i64]
                      + [c_p] * 11,
+    "mr_rec_lexicon_build_bytes": [c_i64],
+    "mr_rec_lexicon_build": [c_p, c_p, c_int, c_p, c_i64, c_p],
+    "mr_rec_measure_workspace_bytes": [c_i64, c_i64, c_i64, c_int],
+    "mr_rec_measure": [c_p, c_int, c_p, c_int, c_p, c_int, c_p, c_int, c_int, c_p, c_p, c_int, c_p, c_p, c_int, c_p, c_p, c_i64]
+                      + [c_p] * 9,
 }
 _RESTYPES = {
     "mr_db_contours_workspace_bytes": c_i64,
@@ -120,6 +125,8 @@ _RESTYPES = {
     "mr_db_boxes_workspace_bytes": c_i64,
     "mr_db_targets_workspace_bytes": c_i64,
     "mr_db_measure_workspace_bytes": c_i64,
+    "mr_rec_lexicon_build_bytes": c_i64,
+    "mr_rec_measure_workspace_bytes": c_i64,
     "mr_db_batch_workspace_bytes": c_i64,
     "mr_db_loss_workspace_bytes": c_i64,
     "mr_dcn_fused_workspace_bytes_h": c_i64,
