@@ -389,6 +389,20 @@ int mr_bias_relu_pool_bwd(const void *dy, const void *y, const unsigned char *id
                           int kw, int sh, int sw, int ph, int pw, int dtype, void *dz, float *dbias, double *sums,
                           void *stream);
 int mr_bias_act(const void *x, const float *bias, int64_t rows, int C, int relu, int dtype, void *y, void *stream);
+/* CRNN stem, backbones/crnn.py layer 0: Conv2d(3, 64, 3, 1, 1) -> ReLU -> MaxPool2d(2, 2) in one kernel each way.
+ * Forward: x NCHW fp32 [N,3,H,W], w [64,3,3,3] / bias [64] fp32 -> y NHWC bf16 [N,H/2,W/2,64] with the rounding of the
+ * unfused bf16 path (z = bf16(conv of bf16 operands), y = maxpool(bf16(relu(z + bias)))); idx (nullable: not written) is
+ * the routing byte per pooled value: i*2 + j of the first arg-max, or 4 when the pooled value is not > 0.
+ * Backward: dw [64,3,3,3] and dbias [64] fp32 from x, dy [N,H/2,W/2,64] bf16 and idx; `sums` = scratch of 1792 doubles.
+ * The two calls give the same bits every time.  The conv stride is (sh, sw), the pool is (pkh, pkw) / (psh, psw) /
+ * (pph, ppw).  MR_ERR_UNSUPPORTED unless Cin = 3, Cout = 64, a 3x3 kernel with stride 1 and padding 1, a 2x2 / 2 pool
+ * without padding and H, W >= 2. */
+int mr_crnn_stem_fwd(const float *x, const float *w, const float *bias, int N, int Cin, int H, int W, int Cout, int kh,
+                     int kw, int sh, int sw, int ph, int pw, int pkh, int pkw, int psh, int psw, int pph, int ppw, void *y,
+                     unsigned char *idx, void *stream);
+int mr_crnn_stem_bwd(const float *x, const void *dy, const unsigned char *idx, int N, int Cin, int H, int W, int Cout,
+                     int kh, int kw, int sh, int sw, int ph, int pw, int pkh, int pkw, int psh, int psw, int pph, int ppw,
+                     float *dw, float *dbias, double *sums, void *stream);
 /* nn.BatchNorm2d in training mode over (x + bias): batch stats, running-stat update, normalise; `sums` = scratch of
  * 2*C doubles.  mr_bn_apply is the eval-mode affine transform with given mean / invstd. */
 int mr_bn_train_fwd(const void *x, const float *bias, const float *gamma, const float *beta, float *running_mean,

@@ -39,6 +39,8 @@ _SIGS = {
     "mr_bias_relu_pool_fwd": [c_p, c_p] + [c_int] * 11 + [c_p, c_p, c_p],
     "mr_bias_relu_pool_bwd": [c_p, c_p, c_p] + [c_int] * 11 + [c_p, c_p, c_p, c_p],
     "mr_bias_act": [c_p, c_p, c_i64, c_int, c_int, c_int, c_p, c_p],
+    "mr_crnn_stem_fwd": [c_p] * 3 + [c_int] * 17 + [c_p] * 3,
+    "mr_crnn_stem_bwd": [c_p] * 3 + [c_int] * 17 + [c_p] * 4,
     "mr_bn_train_fwd": [c_p] * 6 + [c_f32, c_f32, c_i64, c_int, c_int] + [c_p] * 5,
     "mr_bn_apply": [c_p] * 6 + [c_i64, c_int, c_int, c_p, c_p],
     "mr_bn_train_bwd": [c_p] * 6 + [c_i64, c_int, c_int] + [c_p] * 6,

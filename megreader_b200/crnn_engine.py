@@ -6,7 +6,8 @@ The nn.Modules only own parameters (reference names / shapes, SURVEY.md App. C).
     decoders/crnn.py:95-99    log_softmax -> CTC (mean, zero_infinity)
 runs here as two hand-orchestrated autograd Functions over megreader_b200's CUDA kernels: activations stay NHWC
 in the compute dtype (fp32 for parity runs, bf16 for throughput; fp32 accumulation and fp32 master weights in both),
-every convolution is im2col (csrc/nn_kernels.cu) + one dense GEMM (csrc/gemm.cu), bias+ReLU+MaxPool and BatchNorm are
+a convolution is an implicit GEMM (bf16, C % 64 == 0), the fused stem of csrc/crnn_stem.cu (bf16 layer 0 without an
+image gradient) or im2col (csrc/nn_kernels.cu) + one dense GEMM (csrc/gemm.cu), bias+ReLU+MaxPool and BatchNorm are
 single fused passes, the LSTM is one input-projection GEMM per direction plus a per-step recurrent GEMM and a fused
 cell kernel, and the loss is the fused log_softmax+CTC of csrc/ctc2d.cu.  CUDA only: there is no CPU path.
 """
@@ -130,11 +131,22 @@ class _BackboneFn(torch.autograd.Function):
         layers = _conv_layers(module)
         vn = _vn(dtype)
         N, Cin, H, W = x.shape
-        Cp = -(-Cin // vn) * vn
-        a = ops.nchw_to_nhwc(x.contiguous().float(), Cp, dtype)
-        ctx.in_nhwc, ctx.in_channels, ctx.in_dtype = tuple(a.shape), Cin, x.dtype
         saved = []
-        for (conv, bn, pool) in layers:
+        conv0, bn0, pool0 = layers[0]
+        stem = None
+        if dtype == torch.bfloat16 and bn0 is None and pool0 is not None and not ctx.needs_input_grad[0]:
+            # layer 0 (C = 3 is too narrow for the implicit GEMMs) as one fused conv + bias + ReLU + pool kernel reading
+            # the NCHW image; the unfused branch below stays for fp32 and for an image gradient
+            stem = ops.crnn_stem_fwd(x.contiguous().float(), conv0, pool0, save)
+        if stem is not None:
+            a = stem[0]
+            ctx.save_for_backward(x)
+            saved.append({"kind": "stem", "idx": stem[1], "out_hw": tuple(a.shape[1:3])})
+        else:
+            Cp = -(-Cin // vn) * vn
+            a = ops.nchw_to_nhwc(x.contiguous().float(), Cp, dtype)
+            ctx.in_nhwc, ctx.in_channels, ctx.in_dtype = tuple(a.shape), Cin, x.dtype
+        for (conv, bn, pool) in layers[len(saved):]:
             kh, kw = conv.kernel_size
             ph, pw = conv.padding
             assert conv.stride == (1, 1) and conv.dilation == (1, 1) and conv.groups == 1
@@ -200,6 +212,12 @@ class _BackboneFn(torch.autograd.Function):
         for li in range(len(ctx.layers) - 1, -1, -1):
             conv, bn, pool = ctx.layers[li]
             rec = ctx.saved[li]
+            if rec["kind"] == "stem":
+                x, = ctx.saved_tensors
+                dy = dy.view(N, *rec["out_hw"], conv.out_channels)
+                grads = list(ops.crnn_stem_bwd(x.contiguous().float(), dy, rec["idx"], conv, pool)) + grads
+                rec.clear()
+                continue
             Nn, H, W, C = rec["in_shape"]
             Ho, Wo = rec["out_hw"]
             Cout = rec["Wm"].size(0)

@@ -32,6 +32,12 @@ int blas_handle(cublasHandle_t *h, cudaStream_t st);
 int ensure_dyn_smem(const void *func, size_t bytes, const char *where);
 int sm_count();
 
+// Per-block partial sums added in a fixed order (csrc/nn_kernels.cu): block_partials() is the library-owned scratch of
+// `rows` x `cols` floats (NULL when it is smaller or cannot be allocated; its first allocation must not happen during a
+// CUDA-graph capture), finalize_partials() launches partials_finalize_kernel: sums[c] = sum over the rows in double.
+float *block_partials(int rows, int cols);
+int finalize_partials(const float *part, int rows, int cols, double *sums, cudaStream_t st);
+
 inline int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 inline int64_t round_up(int64_t a, int64_t b) { return ceil_div(a, b) * b; }
 

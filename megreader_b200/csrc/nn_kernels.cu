@@ -1243,6 +1243,17 @@ int vec_ok(int dtype, int C) { return C % (dtype == 0 ? 4 : 8) == 0; }
 
 }  // namespace
 
+namespace mr {
+float *block_partials(int rows, int cols) {
+    return (rows <= kMaxPartialBlocks && cols <= kMaxPartialCols) ? partials_scratch() : nullptr;
+}
+
+int finalize_partials(const float *part, int rows, int cols, double *sums, cudaStream_t st) {
+    partials_finalize_kernel<<<(int)ceil_div(cols, 32), dim3(32, 32), 0, st>>>(part, rows, cols, sums);
+    return check_launch("partials_finalize_kernel");
+}
+}  // namespace mr
+
 extern "C" {
 
 int mr_colsum(const void *a, int64_t rows, int C, int dtype, float *out, int accumulate, double *sums, void *stream);

@@ -81,6 +81,38 @@ def bias_relu_pool_bwd(dy, y, idx, N, H, W, C, k, s, p, want_dbias=True):
     return dz, dbias
 
 
+def _stem_geo(conv, pool):
+    """(Cout, kh, kw, sh, sw, ph, pw, pkh, pkw, psh, psw, pph, ppw) of a Conv2d + MaxPool2d pair, as the stem entries take it."""
+    pk, ps, pp = [(v, v) if isinstance(v, int) else tuple(v) for v in (pool.kernel_size, pool.stride, pool.padding)]
+    return (conv.out_channels,) + tuple(conv.kernel_size) + tuple(conv.stride) + tuple(conv.padding) + pk + ps + pp
+
+
+def crnn_stem_fwd(x, conv, pool, save):
+    """CRNN layer 0 (csrc/crnn_stem.cu): x NCHW fp32 -> (y [N, H/2, W/2, 64] bf16 NHWC, routing bytes or None when not
+    `save`).  None when the entry refuses the geometry (MR_ERR_UNSUPPORTED): the caller then takes the unfused path."""
+    N, C, H, W = x.shape
+    geo = _stem_geo(conv, pool)
+    w, b = conv.weight.detach().float().contiguous(), conv.bias.detach().float().contiguous()
+    y = torch.empty((N, H // 2, W // 2, conv.out_channels), dtype=torch.bfloat16, device=x.device)
+    idx = torch.empty(y.shape, dtype=torch.uint8, device=x.device) if save else None
+    rc = _lib.lib().mr_crnn_stem_fwd(_p(x), _p(w), _p(b), N, C, H, W, *geo, _p(y), _p(idx), _st())
+    if rc == _lib.MR_ERR_UNSUPPORTED:
+        return None
+    _chk(rc, "crnn_stem_fwd")
+    return y, idx
+
+
+def crnn_stem_bwd(x, dy, idx, conv, pool):
+    """-> (dW [64, 3, 3, 3], dbias [64]) fp32 of the stem from x NCHW fp32, dy [N, H/2, W/2, 64] bf16 and the routing."""
+    N, C, H, W = x.shape
+    dw = torch.empty(conv.weight.shape, dtype=torch.float32, device=x.device)
+    db = torch.empty((conv.out_channels,), dtype=torch.float32, device=x.device)
+    sums = torch.empty((dw.numel() + db.numel(),), dtype=torch.float64, device=x.device)
+    _chk(_lib.lib().mr_crnn_stem_bwd(_p(x), _p(dy), _p(idx), N, C, H, W, *_stem_geo(conv, pool), _p(dw), _p(db), _p(sums),
+                                     _st()), "crnn_stem_bwd")
+    return dw, db
+
+
 def bias_act(x, bias, relu=False, out=None):
     rows, C = x.shape
     y = out if out is not None else torch.empty_like(x)
