@@ -12,8 +12,15 @@ bf16 NHWC activations).
     share of the step that the convolutions are.
         python benchmarks/crnn_conv_layers.py --profile --out DIR [--steps 3]
 
-Both write JSON into DIR together with the card's name, power limit and maximum SM clock.  L0 (Cin = 3) runs as
-im2col + cuBLAS GEMM and is not an implicit convolution.
+(c) the persistent kernels against each other, call by call, the arms alternating round after round: forward and input
+    gradient on the 128-pixel ping-pong kernel (tile_m=128) and as mr_conv_fprop_pp selects (tile_m=0: the 256-pixel
+    kernel from 36 K blocks on), L6's input gradient also as the engine's row split (two 1 x 2 convolutions), and the
+    weight gradient with the planner's schedule (its old arm is this script's (a) run from the parent build).  Beside
+    TFLOP/s it prints the L2-to-SM rate implied by the kernel's operand bytes per FLOP.
+        python benchmarks/crnn_conv_layers.py --changed --out DIR [--batch 512] [--rounds 3]
+
+All write JSON into DIR together with the card's name, power limit and maximum SM clock.  L0 (Cin = 3) runs on the fused
+stem kernels of csrc/crnn_stem.cu (benchmarks/crnn_stem.py) and is not an implicit convolution.
 """
 import argparse
 import json
@@ -103,6 +110,70 @@ def run_layers(args):
             "total_us": tot}
 
 
+# operand bytes loaded from L2 per FLOP: a 64-deep K block of a 128 x 128 tile (ping-pong), of two 128-pixel tiles sharing
+# one 128-wide weight box (256-pixel kernel), of a 128 x 256 weight-gradient tile (RB rows: the same ratio)
+B_PER_FLOP = {"pp128": 32768 / (2 * 128 * 128 * 64), "m256": 49152 / (2 * 256 * 128 * 64),
+              "wgrad": (128 + 256) * 128 / (2 * 128 * 256 * 64)}
+
+
+def changed_calls(n, dev):
+    """[(layer, kind, flop, {arm: (fn, bytes per FLOP)})] on seeded bf16 operands."""
+    from megreader_b200 import crnn_engine
+    g = torch.Generator(device=dev).manual_seed(0)
+    out = []
+    for name, H, W, C, Cout, k, p in LAYERS:
+        Ho, Wo = H + 2 * p - k + 1, W + 2 * p - k + 1
+        flop = 2.0 * n * Ho * Wo * Cout * k * k * C
+        x = torch.randn((n, H, W, C), generator=g, device=dev).to(torch.bfloat16)
+        Wm = (torch.randn((Cout, k * k * C), generator=g, device=dev) / (k * k * C) ** 0.5).to(torch.bfloat16)
+        dz = torch.randn((n, Ho, Wo, Cout), generator=g, device=dev).to(torch.bfloat16)
+        Wd = (torch.randn((C, k * k * Cout), generator=g, device=dev) / (k * k * Cout) ** 0.5).to(torch.bfloat16)
+        dW = torch.zeros((Cout, k * k * C), dtype=torch.float32, device=dev)
+        for kind, a, w, pad, kb in (("fprop", x, Wm, p, k * k * C // 64), ("dgrad", dz, Wd, k - 1 - p, k * k * Cout // 64)):
+            sel = "m256" if kb >= 36 else "pp128"
+            arms = {"pp128": (lambda a=a, w=w, k=k, pad=pad: ops.conv_fprop_pp(a, w, k, k, pad, pad, tile_m=128)[0],
+                              B_PER_FLOP["pp128"]),
+                    "selected": (lambda a=a, w=w, k=k, pad=pad: ops.conv_fprop_pp(a, w, k, k, pad, pad)[0],
+                                 B_PER_FLOP[sel])}
+            if kind == "dgrad" and Ho == 1:
+                arms["rows"] = (lambda a=a, w=w, k=k, p=p, H=H: crnn_engine._conv_dgrad(a, w, k, k, p, p, H),
+                                B_PER_FLOP["pp128"])
+            out.append((name, kind, flop, arms))
+        out.append((name, "wgrad", flop, {"selected": (lambda dz=dz, x=x, k=k, p=p, dW=dW: ops.conv_wgrad_pp(
+            dz, x, k, k, p, p, out=dW.zero_()), B_PER_FLOP["wgrad"])}))
+    return out
+
+
+def run_changed(args):
+    dev = torch.device("cuda:0")
+    cs = changed_calls(args.batch, dev)
+    times = defaultdict(list)
+    for _ in range(args.rounds):
+        for i, (_, _, _, arms) in enumerate(cs):
+            for arm, (fn, _) in arms.items():
+                times[(i, arm)].append(bench._graph_time(fn, args.iters))
+    rows = []
+    for i, (name, kind, flop, arms) in enumerate(cs):
+        row = {"layer": name, "kind": kind, "gflop": flop * 1e-9}
+        ref = None
+        for arm, (fn, bpf) in arms.items():
+            ts = times[(i, arm)]
+            t = sorted(ts)[len(ts) // 2]
+            row[arm] = {"us": t * 1e6, "us_all": [v * 1e6 for v in ts], "tflops": flop / t * 1e-12,
+                        "l2_tb_s": flop / t * bpf * 1e-12}
+            if kind != "wgrad":
+                r = fn()
+                ref = r.clone() if ref is None else ref
+                row[arm]["same_bits_as_pp128"] = bool(torch.equal(r.view_as(ref), ref))
+        rows.append(row)
+        print("%-3s %-6s %s" % (name, kind, "  ".join(
+            "%s %7.1f us (%s) %6.1f TFLOP/s L2 %4.1f TB/s%s" % (
+                arm, v["us"], "/".join("%.0f" % u for u in v["us_all"]), v["tflops"], v["l2_tb_s"],
+                "" if v.get("same_bits_as_pp128", True) else " DIFFERENT")
+            for arm, v in row.items() if isinstance(v, dict))), flush=True)
+    return {"batch": args.batch, "iters_per_graph": args.iters, "rounds": args.rounds, "calls": rows}
+
+
 def kernel_family(name):
     m = re.match(r"(?:void )?(?:\(anonymous namespace\)::)?([\w:]+?)(?:<|\(|$)", name)
     return m.group(1) if m else name
@@ -156,15 +227,17 @@ def main():
     ap.add_argument("--iters", type=int, default=20, help="launches per CUDA graph")
     ap.add_argument("--rounds", type=int, default=3, help="alternating old / new rounds (the median is reported)")
     ap.add_argument("--profile", action="store_true", help="(b): profile whole training steps instead")
+    ap.add_argument("--changed", action="store_true", help="(c): the persistent kernels against each other")
     ap.add_argument("--steps", type=int, default=3, help="profiled steps for --profile")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("crnn_conv_layers: needs a CUDA device")
     info = card()
-    rec = run_profile(args) if args.profile else run_layers(args)
+    rec = run_profile(args) if args.profile else run_changed(args) if args.changed else run_layers(args)
     rec["card"] = info
     os.makedirs(args.out, exist_ok=True)
-    path = os.path.join(args.out, "crnn_conv_profile.json" if args.profile else "crnn_conv_layers.json")
+    path = os.path.join(args.out, "crnn_conv_profile.json" if args.profile else
+                        "crnn_conv_changed.json" if args.changed else "crnn_conv_layers.json")
     with open(path, "w") as f:
         json.dump(rec, f, indent=1)
     print("card: %s" % json.dumps(info))

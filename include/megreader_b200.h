@@ -462,19 +462,23 @@ int mr_conv2d_wgrad_tcgen05(const void *dz, const void *x, float *dWm, int N, in
 /* Implicit-GEMM weight gradient: dWm[Cout, kh*kw*C] fp32 += dz[N,Ho,Wo,Cout]^T (*) x[N,H,W,C] (atomic, split-K). */
 int mr_conv_wgrad_tcgen05(const void *dz, const void *x, float *dWm, int N, int H, int W, int C, int Cout, int kh, int kw,
                           int ph, int pw, int splits, void *stream);
-/* The CRNN backbone's convolutions on persistent ping-pong wgmma kernels (csrc/conv_pingpong.cu): stride 1, NHWC bf16 ->
- * bf16, no bias or activation.  y[N*Ho*Wo, Cout] = conv(x[N,H,W,C], Wm[Cout, kh*kw*C]), bit-identical to
- * mr_conv_fprop_tcgen05's bf16 output; with flipped/transposed weights and padding (k-1-p) the input gradient.
- * MR_ERR_UNSUPPORTED unless C % 64 == 0, Cout % 8 == 0, 16-byte aligned pointers and an output that tiles with at most
- * four TMA box segments (the caller then uses mr_conv_fprop_tcgen05). */
+/* The CRNN backbone's convolutions on persistent wgmma kernels (csrc/conv_pingpong.cu): stride 1, NHWC bf16 -> bf16, no
+ * bias or activation.  y[N*Ho*Wo, Cout] = conv(x[N,H,W,C], Wm[Cout, kh*kw*C]), bit-identical to mr_conv_fprop_tcgen05's
+ * bf16 output; with flipped/transposed weights and padding (k-1-p) the input gradient.  ldw: elements between Wm's rows
+ * (0: kh*kw*C); y_nstride: elements between y's images (0: Ho*Wo*Cout).  tile_m: 128 the ping-pong kernel with 128-pixel
+ * tiles, 256 the kernel with 256-pixel tiles sharing one weight stage (Cout > 64), 0 the one chosen by the K-block count (256 from 36 on).
+ * MR_ERR_UNSUPPORTED unless C % 64 == 0, Cout % 8 == 0, 16-byte aligned pointers, strides that are multiples of 8 and an
+ * output that tiles with at most four TMA box segments (the caller then uses mr_conv_fprop_tcgen05). */
 int mr_conv_fprop_pp(const void *x, const void *Wm, void *y, int N, int H, int W, int C, int Cout, int kh, int kw, int ph,
-                     int pw, void *stream);
+                     int pw, int ldw, int y_nstride, int tile_m, void *stream);
 /* Weight gradient of the same convolutions on a persistent wgmma kernel with 128 x 256 tiles (csrc/conv_pingpong.cu):
  * dWm[Cout, kh*kw*C] fp32 += dz[N,Ho,Wo,Cout]^T (*) x[N,H,W,C], ACCUMULATED atomically (zero it first).  The K blocks of
- * all tiles are split evenly over `ctas` CTAs (<= 0: one per SM).  MR_ERR_UNSUPPORTED unless C % 64 == 0, Cout % 8 == 0
- * and 16-byte aligned pointers (the caller then uses mr_conv_wgrad_tcgen05). */
+ * all tiles are cut into splits, and the (split, tile) units are handed out to at most `ctas` CTAs (<= 0: one per SM),
+ * an equal number each where a grid of at least 90 % of `ctas` allows it; a split keeps at least `min_kb` K blocks where
+ * the plan allows it.  MR_ERR_UNSUPPORTED unless C % 64 == 0, Cout % 8 == 0 and 16-byte aligned pointers (the caller then
+ * uses mr_conv_wgrad_tcgen05). */
 int mr_conv_wgrad_pp(const void *dz, const void *x, float *dWm, int N, int H, int W, int C, int Cout, int kh, int kw, int ph,
-                     int pw, int ctas, void *stream);
+                     int pw, int ctas, int min_kb, void *stream);
 
 /* Fused LSTM time steps on wgmma (recurrent GEMM + cell in one launch, both directions): gate columns are
  * UNIT-MAJOR (column 4*j + g = gate g in {i,f,g,o} of hidden unit j), H % 64 == 0, bf16.  Every per-direction argument

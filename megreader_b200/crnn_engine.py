@@ -115,6 +115,25 @@ def _conv_fprop(x, Wm, kh, kw, ph, pw):
     return r if r is not None else ops.conv_fprop_tc(x, Wm, kh, kw, ph, pw)
 
 
+def _conv_dgrad(dz, Wd, kh, kw, ph, pw, H):
+    """Input gradient [N*H*W, C] of a stride-1 convolution with padding (ph, pw): dz [N,Ho,Wo,Cout] convolved with the
+    flipped, transposed weights Wd [C, kh*kw*Cout] and padding k-1-p.  With a one-row dz (L6: 2 x 2 kernel, padding 0)
+    every dx row meets exactly one real tap row and the others only padding, so each row is computed as a 1 x kw
+    convolution with that tap row's weights, stored into its row of dx: half the MMA work at L6, and the same bits, since
+    the skipped taps only add exact zeros."""
+    N, Ho, Wo, Cout = dz.shape
+    if Ho == 1 and kh > 1:
+        dx = torch.empty((N, H, Wo + kw - 1 - 2 * pw, Wd.size(0)), dtype=dz.dtype, device=dz.device)
+        row = kw * Cout
+        for r in range(H):
+            i = kh - 1 - ph - r                           # the flipped tap row that meets dz's row
+            if ops.conv_fprop_pp(dz, Wd[:, i * row:(i + 1) * row], 1, kw, 0, kw - 1 - pw, out=dx[:, r:r + 1]) is None:
+                break
+        else:
+            return dx.view(-1, dx.size(3))
+    return _conv_fprop(dz, Wd, kh, kw, kh - 1 - ph, kw - 1 - pw)[0]
+
+
 def _conv_wgrad(dz, x, kh, kw, ph, pw, out=None):
     """Weight gradient [Cout, kh*kw*C] fp32 (accumulated into a zeroed `out` if given) on the persistent 128 x 256 kernel;
     the one-tile-per-CTA kernel only for geometries the former refuses."""
@@ -265,7 +284,7 @@ class _BackboneFn(torch.autograd.Function):
                         Wd = ops.conv_weight_pack(wsrc, C, kh * kw * C, dtype, 1)          # flipped + transposed, one launch
                     else:
                         Wd = ops.cast(wsrc.flip(2, 3).permute(1, 2, 3, 0).reshape(C, kh * kw * Cout).contiguous(), dtype)
-                    dy, _, _ = _conv_fprop(dz4, Wd, kh, kw, kh - 1 - ph, kw - 1 - pw)
+                    dy = _conv_dgrad(dz4, Wd, kh, kw, ph, pw, H)
                 else:
                     dcol = ops.gemm(dz, rec["Wm"])                                           # [P, Kp]
                     dy = ops.col2im(dcol, Nn, H, W, C, kh, kw, ph, pw).view(Nn * H * W, C)

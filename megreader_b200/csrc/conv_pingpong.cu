@@ -22,6 +22,7 @@
 // bit-identical.
 #include "wgmma.cuh"
 #include <algorithm>
+#include <numeric>
 
 namespace {
 
@@ -32,6 +33,11 @@ static_assert(128 * kPpProducerRegs + 256 * kPpConsumerRegs <= 65536, "register 
 
 // Named barriers (0 is __syncthreads): the consumers' turn barriers, and one per consumer for its epilogue.
 constexpr int kBarTurn0 = 1, kBarTurn1 = 2, kBarEpi0 = 3;
+
+// K blocks (64 deep) from which mr_conv_fprop_pp picks conv_fprop_m256_kernel over conv_fprop_pp_kernel.  On an H100 SXM
+// the 256-pixel tiles were faster at 36 K blocks (L3 forward, L2 input gradient at batch 512) and 2 % slower at 32 (L6
+// forward), where the ping-pong kernel's overlap of one consumer's epilogue with the other's main loop matters more.
+constexpr int kM256MinKb = 36;
 
 // STAGES x (A 128x64, B BNx64) from a 1024-byte aligned base, then one bf16 output tile per consumer (BN/64 slices of
 // 128 rows x 128 B, the TMA store boxes), then the barriers full[STAGES], empty[STAGES].
@@ -50,7 +56,7 @@ template <int BN> struct PpSmem {
 
 struct PpConvArgs {
     int C, Cout, kh, kw, ph, pw;
-    int cout_tiles, tiles;            // tiles = 128-pixel tiles x cout_tiles
+    int pix_tiles, cout_tiles, tiles; // tiles = 128-pixel tiles (pairs of them for conv_fprop_m256_kernel) x cout_tiles
     int nseg;
     ConvSeg seg[kMaxConvSegs];
 };
@@ -195,33 +201,177 @@ conv_fprop_pp_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_const
 }
 
 // =====================================================================================================
+// Large-K variant (kM256MinKb): a CTA tile is two consecutive 128-pixel tiles x one BN-wide Cout tile.  A stage holds both activation
+// boxes (each from its own segment's tensor map) and ONE weight box, and consumer c multiplies activation box c by it, so
+// the CTA loads 48 KB per 4.2 MFLOP instead of conv_fprop_pp_kernel's 32 KB per 2.1 MFLOP.  Each consumer's accumulator,
+// K order, instruction sequence and epilogue are those of conv_fprop_pp_kernel<BN>: the output is the same bits.  Both
+// consumers work on the same stage at once (its empty barrier takes two arrivals), so there is no turn order and no
+// epilogue overlap inside the CTA; the producer keeps filling the ring while the consumers store.  An odd last pixel tile
+// leaves consumer 1 without a tile: it stores nothing but still consumes every stage, whose second box the producer loads
+// entirely out of bounds (zero fill) to keep the transaction count.
+// =====================================================================================================
+template <int BN> struct M256Smem {
+    static constexpr int STAGES = 3;
+    static constexpr int A_BYTES = BM * BK * 2;            // one 128-pixel activation box
+    static constexpr int B_BYTES = BN * BK * 2;
+    static constexpr int STAGE_BYTES = 2 * A_BYTES + B_BYTES;
+    static constexpr int SLICE_BYTES = BM * 64 * 2;
+    static constexpr int OUT_BYTES = (BN / 64) * SLICE_BYTES;
+    static constexpr int OUT_OFF = STAGES * STAGE_BYTES;
+    static constexpr int BAR_OFF = OUT_OFF + 2 * OUT_BYTES;
+    static constexpr int TOTAL = BAR_OFF + 2 * STAGES * 8 + 1024;
+    static_assert(TOTAL <= 232448, "227 KB of opt-in shared memory");
+};
+
+template <int BN>
+__global__ void __launch_bounds__(kPpThreads, 1)
+conv_fprop_m256_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmX0,
+                       const __grid_constant__ CUtensorMap tmX1, const __grid_constant__ CUtensorMap tmX2,
+                       const __grid_constant__ CUtensorMap tmX3, const __grid_constant__ CUtensorMap tmY0,
+                       const __grid_constant__ CUtensorMap tmY1, const __grid_constant__ CUtensorMap tmY2,
+                       const __grid_constant__ CUtensorMap tmY3, const __grid_constant__ PpConvArgs a) {
+    using L = M256Smem<BN>;
+    constexpr int STAGES = L::STAGES;
+    extern __shared__ unsigned char smem_raw[];
+    unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
+    uint64_t *empty = full + STAGES;
+    const int wg = threadIdx.x >> 7;
+    const int cchunks = a.C / BK;
+    const int nkb = a.kh * a.kw * cchunks;
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tmB);
+        tma_prefetch_desc(&tmX0);
+        tma_prefetch_desc(&tmY0);
+        for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 2); }   // empty: both consumers
+        fence_barrier_init();
+    }
+    __syncthreads();
+
+    if (wg == 0) {
+        // ------------------------------------------------------------ producer
+        reg_dec<kPpProducerRegs>();
+        if (threadIdx.x < 32 && elect_one()) {
+            uint32_t it = 0;
+            for (int t = blockIdx.x; t < a.tiles; t += gridDim.x) {
+                const int pair = t / a.cout_tiles;
+                const int n0 = (t - pair * a.cout_tiles) * BN;
+                const bool two = 2 * pair + 1 < a.pix_tiles;
+                const PixTile p0 = pix_tile(a, 2 * pair);
+                const PixTile p1 = two ? pix_tile(a, 2 * pair + 1) : p0;
+                const CUtensorMap *tx0 = p0.sel == 0 ? &tmX0 : (p0.sel == 1 ? &tmX1 : (p0.sel == 2 ? &tmX2 : &tmX3));
+                const CUtensorMap *tx1 = p1.sel == 0 ? &tmX0 : (p1.sel == 1 ? &tmX1 : (p1.sel == 2 ? &tmX2 : &tmX3));
+                // no second tile: a box wholly left of the tensor (w + box width <= 0), all zero fill
+                const int w1 = two ? p1.w0 - a.pw : -256;
+                int cc = 0, ti = 0, tj = 0;
+                for (int i = 0; i < nkb; ++i, ++it) {
+                    const int s = it % STAGES;
+                    mbar_wait(empty + s, ((it / STAGES) & 1) ^ 1);
+                    unsigned char *dst = smem + s * L::STAGE_BYTES;
+                    mbar_expect_tx(full + s, L::STAGE_BYTES);
+                    tma_load_4d(tx0, full + s, dst, cc * BK, p0.w0 + tj - a.pw, p0.h0 + ti - a.ph, p0.n);
+                    tma_load_4d(tx1, full + s, dst + L::A_BYTES, cc * BK, w1 + (two ? tj : 0), p1.h0 + ti - a.ph, p1.n);
+                    tma_load_2d(&tmB, full + s, dst + 2 * L::A_BYTES, i * BK, n0);
+                    if (++cc == cchunks) { cc = 0; if (++tj == a.kw) { tj = 0; ++ti; } }
+                }
+            }
+        }
+        return;
+    }
+
+    // ---------------------------------------------------------------- consumers: pixel tile c of every pair
+    reg_inc<kPpConsumerRegs>();
+    const int c = wg - 1;
+    const int mt = threadIdx.x & 127;
+    const int w = mt >> 5, l = mt & 31;
+    unsigned char *out = smem + L::OUT_OFF + c * L::OUT_BYTES;
+    const uint32_t out_addr = smem_u32(out);
+    uint32_t it0 = 0;                                          // ring position of the tile's first K block
+    for (int t = blockIdx.x; t < a.tiles; t += gridDim.x, it0 += nkb) {
+        AccTile<BN> acc;
+        for (int i = 0; i < nkb; ++i) {
+            const uint32_t it = it0 + i;
+            const int s = it % STAGES;
+            mbar_wait(full + s, (it / STAGES) & 1);
+            wgmma_fence();
+            const uint32_t a_addr = smem_u32(smem + s * L::STAGE_BYTES + c * L::A_BYTES);
+            const uint32_t b_addr = smem_u32(smem + s * L::STAGE_BYTES + 2 * L::A_BYTES);
+#pragma unroll
+            for (int kk = 0; kk < BK / WGMMA_K; ++kk)
+                acc.template mma<0, 0>(desc_kmajor(a_addr, kk), desc_kmajor(a_addr, kk, 1), desc_kmajor(b_addr, kk),
+                                       (i | kk) != 0);
+            wgmma_commit();
+            wgmma_wait<1>();                                   // block i - 1 has retired: hand its stage back
+            if (i > 0 && mt == 0) mbar_arrive(empty + (it - 1) % STAGES);
+        }
+        wgmma_wait<0>();
+        if (mt == 0) mbar_arrive(empty + (it0 + nkb - 1) % STAGES);
+
+        // ------------------------------------------------------------ epilogue: as conv_fprop_pp_kernel's
+        const int pair = t / a.cout_tiles;
+        const int n0 = (t - pair * a.cout_tiles) * BN;
+        const int pt = 2 * pair + c;
+        if (pt >= a.pix_tiles) continue;                       // consumer 1 of an odd last pair
+        if (mt == 0) bulk_wait_group_read<0>();                // the previous tile's stores have read the staging tile
+        named_bar_sync<128>(kBarEpi0 + c);
+        const int sub = l >> 3, rr = l & 7;
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+            const int row = half * 64 + 16 * w + 8 * (sub & 1) + rr;
+#pragma unroll
+            for (int j = 0; j < BN / 8; j += 2) {
+                const int q = j >> 3, chunk = (j & 7) + (sub >> 1);
+                const uint32_t addr = out_addr + q * L::SLICE_BYTES + row * 128 + ((chunk ^ (row & 7)) << 4);
+                uint32_t r[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    __nv_bfloat162 h2 = __floats2bfloat162_rn(acc.d[half][4 * j + 2 * e], acc.d[half][4 * j + 2 * e + 1]);
+                    r[e] = *reinterpret_cast<uint32_t *>(&h2);
+                }
+                stmatrix_x4(addr, r[0], r[1], r[2], r[3]);
+            }
+        }
+        fence_proxy_async();                                   // generic-proxy smem writes -> visible to the TMA store
+        named_bar_sync<128>(kBarEpi0 + c);
+        if (mt == 0) {
+            const PixTile p = pix_tile(a, pt);
+            const CUtensorMap *tmY = p.sel == 0 ? &tmY0 : (p.sel == 1 ? &tmY1 : (p.sel == 2 ? &tmY2 : &tmY3));
+#pragma unroll
+            for (int q = 0; q < BN / 64; ++q)
+                if (n0 + 64 * q < a.Cout) tma_store_4d(tmY, out + q * L::SLICE_BYTES, n0 + 64 * q, p.w0, p.h0, p.n);
+            bulk_commit_group();
+        }
+    }
+    if (mt == 0) bulk_wait_group<0>();                         // the staging tile must outlive the last store's reads
+}
+
+// =====================================================================================================
 // Persistent implicit-GEMM weight gradient:  dW[co, tap*C + c] += sum_p dz[p, co] * x[pixel(p) shifted by tap, c]
 //
 // CTA tile 128 (Cout) x 256 (kh*kw*C columns): both consumer warpgroups read the same dz (A) stage and each owns one
 // 128-column half of the x (B) operand, so a stage of dz is loaded once per 256 columns.  Both operands come MN-major by
 // 4-D TMA exactly as in conv_wgrad_tcgen05_kernel (K block = RB output pixels of one row; tap shift = signed coordinate
-// offset, padding = TMA zero fill).  The work is split stream-K: the iterations of the whole problem, ordered as (split,
-// tile, K block of the split), are cut into gridDim.x equal contiguous ranges, one per CTA, so every SM gets the same number
-// of K blocks whatever the tile count.  With splits ~ gridDim.x / tiles the CTAs that run side by side work on the same
-// split, i.e. on the same rows of dz and x, which are then read from HBM once and hit in L2 by the other tiles.  A CTA accumulates each tile's part of its range in registers and adds it into dW (pre-zeroed by the caller)
-// straight from the fragments with red.global.add.v4.f32.
+// offset, padding = TMA zero fill).  The K blocks are cut into `splits` equal splits; a unit is one (split, tile), and the
+// units, numbered split-major, are handed out strided by gridDim.x.  The planner makes the unit count a whole multiple of
+// the grid, so every CTA gets the same number of units, and the CTAs that run side by side work on one split or on
+// adjacent ones, i.e. on the same rows of dz and x, which are then read from HBM once and hit in L2 by the other tiles.  A
+// CTA accumulates a unit in registers and adds it into dW (pre-zeroed by the caller) straight from the fragments with
+// red.global.add.v4.f32.
 // =====================================================================================================
 struct PpWgradArgs {
     int C, Cout, K, kw, ph, pw, Ho, wboxes;
     int kb_total, n_tiles, tiles;     // K blocks per tile; 256-column tiles per 128-row block; all tiles
-    int kb_split;                     // K blocks per split
-    int total, per;                   // splits x tiles x kb_split iterations, per CTA
+    int kb_split;                     // K blocks per split (the last split may be shorter, or empty)
+    int units;                        // splits x tiles
 };
 
-// The part of [g, g_end) that lies in one (split, tile): K blocks [kb_lo, kb_hi) of `tile` (empty past the last K block of
-// a short last split) and the `len` iterations it spans.
-struct WgradSeg { int tile, kb_lo, kb_hi, len; };
-__device__ __forceinline__ WgradSeg wgrad_seg(const PpWgradArgs &a, int g, int g_end) {
-    const int u = g / a.kb_split, kk = g - u * a.kb_split;
+// Unit u = (split u / tiles, tile u % tiles): K blocks [kb_lo, kb_hi) of `tile`.
+struct WgradUnit { int tile, kb_lo, kb_hi; };
+__device__ __forceinline__ WgradUnit wgrad_unit(const PpWgradArgs &a, int u) {
     const int sp = u / a.tiles;
-    const int len = min(a.kb_split - kk, g_end - g);
-    const int lo = sp * a.kb_split + kk;
-    return {u - sp * a.tiles, min(lo, a.kb_total), min(lo + len, a.kb_total), len};
+    const int lo = min(sp * a.kb_split, a.kb_total);
+    return {u - sp * a.tiles, lo, min(lo + a.kb_split, a.kb_total)};
 }
 
 template <int RB> struct PpWgradSmem {
@@ -250,8 +400,6 @@ conv_wgrad_pp_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_cons
     uint64_t *full = (uint64_t *)(smem + L::BAR_OFF);
     uint64_t *empty = full + STAGES;
     const int wg = threadIdx.x >> 7;
-    const int g_begin = (int)blockIdx.x * a.per;
-    const int g_end = min(a.total, g_begin + a.per);
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmDz);
@@ -266,10 +414,9 @@ conv_wgrad_pp_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_cons
         reg_dec<kPpProducerRegs>();
         if (threadIdx.x < 32 && elect_one()) {
             uint32_t it = 0;
-            for (int g = g_begin; g < g_end;) {
-                const WgradSeg sg = wgrad_seg(a, g, g_end);
-                g += sg.len;
-                const int tile = sg.tile, kb_lo = sg.kb_lo, kb_hi = sg.kb_hi;
+            for (int u = blockIdx.x; u < a.units; u += gridDim.x) {
+                const WgradUnit un = wgrad_unit(a, u);
+                const int tile = un.tile, kb_lo = un.kb_lo, kb_hi = un.kb_hi;
                 const int mt = tile / a.n_tiles;
                 const int m0 = mt * BM, n0 = (tile - mt * a.n_tiles) * 256;
                 int at_i[4], at_j[4], at_c[4];                 // the 4 column atoms of this tile: (tap, channel offset)
@@ -314,10 +461,9 @@ conv_wgrad_pp_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_cons
     const int w = mt_ >> 5, l = mt_ & 31;
     const bool odd = l & 1;
     uint32_t it = 0;
-    for (int g = g_begin; g < g_end;) {
-        const WgradSeg sg = wgrad_seg(a, g, g_end);
-        g += sg.len;
-        const int tile = sg.tile, nkb = sg.kb_hi - sg.kb_lo;
+    for (int u = blockIdx.x; u < a.units; u += gridDim.x) {
+        const WgradUnit un = wgrad_unit(a, u);
+        const int tile = un.tile, nkb = un.kb_hi - un.kb_lo;
         if (nkb == 0) continue;
         const int mt = tile / a.n_tiles;
         const int m0 = mt * BM, n0 = (tile - mt * a.n_tiles) * 256 + c * 128;
@@ -368,6 +514,15 @@ int launch_pp(const CUtensorMap &tb, const CUtensorMap *tx, const CUtensorMap *t
     return check_launch("conv_fprop_pp_kernel");
 }
 
+template <int BN>
+int launch_m256(const CUtensorMap &tb, const CUtensorMap *tx, const CUtensorMap *ty, const PpConvArgs &a, int grid,
+                cudaStream_t st) {
+    auto kern = conv_fprop_m256_kernel<BN>;
+    { int rc = ensure_dyn_smem((const void *)kern, M256Smem<BN>::TOTAL, "conv_fprop_m256 smem attr"); if (rc) return rc; }
+    kern<<<grid, kPpThreads, M256Smem<BN>::TOTAL, st>>>(tb, tx[0], tx[1], tx[2], tx[3], ty[0], ty[1], ty[2], ty[3], a);
+    return check_launch("conv_fprop_m256_kernel");
+}
+
 template <int RB>
 int launch_wgrad_pp(const CUtensorMap &tdz, const CUtensorMap &tx, float *dW, const PpWgradArgs &a, int grid,
                     cudaStream_t st) {
@@ -381,19 +536,31 @@ int launch_wgrad_pp(const CUtensorMap &tdz, const CUtensorMap &tx, float *dW, co
 
 extern "C" {
 
-/* Persistent ping-pong implicit-GEMM stride-1 convolution on NHWC bf16: y[N*Ho*Wo, Cout] bf16 = conv(x[N,H,W,C],
- * Wm[Cout, kh*kw*C]); no bias, no activation.  With flipped/transposed weights and padding (k-1-p) it is the input
- * gradient.  Bit-identical to mr_conv_fprop_tcgen05 with a bf16 output.  MR_ERR_UNSUPPORTED unless C % 64 == 0,
- * Cout % 8 == 0, the pointers are 16-byte aligned and the output tiles with at most four TMA box segments. */
+/* Persistent implicit-GEMM stride-1 convolution on NHWC bf16: y[N*Ho*Wo, Cout] bf16 = conv(x[N,H,W,C], Wm[Cout, kh*kw*C]);
+ * no bias, no activation.  With flipped/transposed weights and padding (k-1-p) it is the input gradient.  Wm's rows are
+ * ldw elements apart (0: kh*kw*C), and y's images y_nstride elements apart (0: Ho*Wo*Cout), so a call can read a column
+ * slice of a wider weight matrix and write rows of a taller output.  tile_m picks the kernel: 128 conv_fprop_pp_kernel,
+ * 256 conv_fprop_m256_kernel (Cout > 64 only), 0 the faster one for the call, by its K-block count.  Bit-identical to
+ * mr_conv_fprop_tcgen05 with a bf16 output whichever runs.  MR_ERR_UNSUPPORTED unless C % 64 == 0, Cout % 8 == 0, the
+ * pointers are 16-byte aligned, the strides are multiples of 8 elements and the output tiles with at most four TMA box
+ * segments. */
 int mr_conv_fprop_pp(const void *x, const void *Wm, void *y, int N, int H, int W, int C, int Cout, int kh, int kw, int ph,
-                     int pw, void *stream) {
+                     int pw, int ldw, int y_nstride, int tile_m, void *stream) {
     if (N < 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0 || kh <= 0 || kw <= 0 || ph < 0 || pw < 0) return MR_ERR_BAD_SHAPE;
     const int Ho = H + 2 * ph - kh + 1, Wo = W + 2 * pw - kw + 1;
     if (Ho <= 0 || Wo <= 0) return MR_ERR_BAD_SHAPE;
+    const int64_t K = (int64_t)kh * kw * C;
+    if (ldw == 0) ldw = (int)K;
+    if (ldw < K || (y_nstride != 0 && y_nstride < (int64_t)Ho * Wo * Cout)) return MR_ERR_BAD_SHAPE;
+    if (tile_m != 0 && tile_m != 128 && tile_m != 256) return MR_ERR_BAD_SHAPE;
     if (N == 0) return MR_OK;
     if (!x || !Wm || !y) return MR_ERR_NULL_POINTER;
     if (C % 64 || Cout % 8 || ((uintptr_t)x % 16) || ((uintptr_t)Wm % 16) || ((uintptr_t)y % 16)) return MR_ERR_UNSUPPORTED;
+    if (ldw % 8 || y_nstride % 8) return MR_ERR_UNSUPPORTED;
     if ((int64_t)N * Ho * Wo > (1LL << 31) - 256) return MR_ERR_UNSUPPORTED;
+    const int BN = Cout > 64 ? 128 : 64;
+    const bool m256 = tile_m == 256 || (tile_m == 0 && K / BK >= kM256MinKb);
+    if (m256 && BN != 128) return MR_ERR_UNSUPPORTED;
     PpConvArgs a;
     a.C = C; a.Cout = Cout; a.kh = kh; a.kw = kw; a.ph = ph; a.pw = pw;
     CUtensorMap tx[kMaxConvSegs], ty[kMaxConvSegs];
@@ -402,31 +569,32 @@ int mr_conv_fprop_pp(const void *x, const void *Wm, void *y, int N, int H, int W
     if (rc) return rc;
     if (a.nseg == 0) return MR_ERR_UNSUPPORTED;
     for (int q = 0; q < a.nseg; ++q) {
-        rc = make_map_nhwc(&ty[q], y, Cout, Wo, Ho, N, a.seg[q].bw, a.seg[q].bh, a.seg[q].bn);
+        rc = make_map_nhwc(&ty[q], y, Cout, Wo, Ho, N, a.seg[q].bw, a.seg[q].bh, a.seg[q].bn, 1, 1, y_nstride);
         if (rc) return rc;
     }
     for (int q = a.nseg; q < kMaxConvSegs; ++q) { tx[q] = tx[0]; ty[q] = ty[0]; }
-    const int BN = Cout > 64 ? 128 : 64;
-    const int64_t K = (int64_t)kh * kw * C;
     CUtensorMap tb;
-    rc = make_map(&tb, Wm, K, Cout, K, BK, BN);
+    rc = make_map(&tb, Wm, K, Cout, ldw, BK, BN);
     if (rc) return rc;
+    a.pix_tiles = pixel_tiles;
     a.cout_tiles = (int)ceil_div(Cout, BN);
-    const int64_t tiles = (int64_t)pixel_tiles * a.cout_tiles;
+    const int64_t tiles = (m256 ? ceil_div(pixel_tiles, 2) : (int64_t)pixel_tiles) * a.cout_tiles;
     if (tiles > (1LL << 31) - 1) return MR_ERR_UNSUPPORTED;
     a.tiles = (int)tiles;
     const int sms = sm_count();
     if (sms <= 0) { set_cuda_error(cudaErrorUnknown, "multiprocessor count"); return MR_ERR_CUDA; }
     const int grid = (int)(tiles < sms ? tiles : sms);
     cudaStream_t st = (cudaStream_t)stream;
+    if (m256) return launch_m256<128>(tb, tx, ty, a, grid, st);
     return BN == 128 ? launch_pp<128>(tb, tx, ty, a, grid, st) : launch_pp<64>(tb, tx, ty, a, grid, st);
 }
 
 /* Persistent implicit-GEMM weight gradient, stride 1: dWm[Cout, kh*kw*C] fp32 (ACCUMULATED atomically: zero it first) from
- * dz[N,Ho,Wo,Cout] and x[N,H,W,C] (NHWC bf16).  The tiles' K blocks are split evenly over `ctas` CTAs (clamped to
- * [1, min(SM count, K blocks)]).  MR_ERR_UNSUPPORTED unless C % 64 == 0, Cout % 8 == 0 and 16-byte aligned operands. */
+ * dz[N,Ho,Wo,Cout] and x[N,H,W,C] (NHWC bf16) on at most `ctas` CTAs (<= 0 or more than the SMs: one per SM), with at least
+ * `min_kb` K blocks per split where the plan allows it.  MR_ERR_UNSUPPORTED unless C % 64 == 0, Cout % 8 == 0 and 16-byte
+ * aligned operands. */
 int mr_conv_wgrad_pp(const void *dz, const void *x, float *dWm, int N, int H, int W, int C, int Cout, int kh, int kw, int ph,
-                     int pw, int ctas, void *stream) {
+                     int pw, int ctas, int min_kb, void *stream) {
     if (N < 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0 || kh <= 0 || kw <= 0 || ph < 0 || pw < 0) return MR_ERR_BAD_SHAPE;
     const int Ho = H + 2 * ph - kh + 1, Wo = W + 2 * pw - kw + 1;
     if (Ho <= 0 || Wo <= 0) return MR_ERR_BAD_SHAPE;
@@ -447,21 +615,33 @@ int mr_conv_wgrad_pp(const void *dz, const void *x, float *dWm, int N, int H, in
     const int sms = sm_count();
     if (ctas <= 0 || ctas > sms) ctas = sms;
     if (ctas > kb_total * tiles) ctas = (int)(kb_total * tiles);
-    const int splits = (int)std::min<int64_t>(kb_total, std::max<int64_t>(1, ctas / tiles));
-    /* When splits x tiles CTAs still fill 90 % of the requested ones, give each CTA exactly one (split, tile): the CTAs
-     * then all sit at the same K offset of their split and read the same dz / x rows at the same time. */
-    if (splits > 1 && (int64_t)splits * tiles * 10 >= (int64_t)ctas * 9) ctas = splits * (int)tiles;
+    if (min_kb < 1) min_kb = 1;
+    /* The plan makes splits x tiles a whole multiple of the grid, and lets the grid go down to 90 % of `ctas` for it:
+     * (1) one unit per CTA, splits = ctas / tiles, when that fills 90 % of the CTAs;
+     * (2) otherwise the largest such grid g whose fewest splits, g / gcd(g, tiles), keep min_kb K blocks each;
+     * (3) otherwise (few K blocks, or few CTAs) ctas / tiles splits, as many as min_kb allows, and some CTAs get one unit
+     *     more than others. */
+    int64_t splits = std::min<int64_t>(kb_total, std::max<int64_t>(1, ctas / tiles));
+    int64_t grid = 0;
+    if (splits * tiles <= ctas && splits * tiles * 10 >= (int64_t)ctas * 9) grid = splits * tiles;
+    for (int g = ctas; grid == 0 && (int64_t)g * 10 >= (int64_t)ctas * 9; --g) {
+        const int64_t s = g / std::gcd<int64_t>(g, tiles);
+        if (kb_total >= s * min_kb) { splits = s; grid = g; }
+    }
+    if (grid == 0) {
+        splits = std::max<int64_t>(1, std::min<int64_t>(splits, kb_total / min_kb));
+        grid = std::min<int64_t>(ctas, splits * tiles);
+    }
     a.kb_split = (int)ceil_div(kb_total, splits);
-    a.total = splits * a.tiles * a.kb_split;
-    a.per = (int)ceil_div(a.total, ctas);
-    const int grid = (int)ceil_div(a.total, a.per);
+    a.units = (int)(splits * tiles);
     CUtensorMap tdz, tx;
     int rc = make_map_nhwc(&tdz, dz, Cout, Wo, Ho, N, RB);
     if (rc) return rc;
     rc = make_map_nhwc(&tx, x, C, W, H, N, RB);
     if (rc) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    return rb80 ? launch_wgrad_pp<80>(tdz, tx, dWm, a, grid, st) : launch_wgrad_pp<64>(tdz, tx, dWm, a, grid, st);
+    return rb80 ? launch_wgrad_pp<80>(tdz, tx, dWm, a, (int)grid, st)
+                : launch_wgrad_pp<64>(tdz, tx, dWm, a, (int)grid, st);
 }
 
 }  // extern "C"

@@ -349,12 +349,13 @@ int make_map(CUtensorMap *m, const void *base, int64_t inner, int64_t outer, int
 // 4-D bf16 NHWC tensor map {C, W, H, N}, box {64, box_w, box_h, box_n}
 // sw / sh > 1: strided traversal (every sw-th column, sh-th row) -- the box then spans box_w * sw columns of the tensor and
 // delivers box_w of them (cuTensorMapEncodeTiled elementStrides)
+// n_stride: elements from one image to the next (0: H * W * C, a dense tensor)
 int make_map_nhwc(CUtensorMap *m, const void *base, int64_t C, int64_t W, int64_t H, int64_t N, int box_w, int box_h = 1,
-                  int box_n = 1, int sw = 1, int sh = 1) {
+                  int box_n = 1, int sw = 1, int sh = 1, int64_t n_stride = 0) {
     EncodeTiledFn fn = encode_fn();
     if (!fn) { set_cuda_error(cudaErrorUnknown, "cuTensorMapEncodeTiled entry point"); return MR_ERR_CUDA; }
     cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)(n_stride ? n_stride : H * W * C) * 2};
     cuuint32_t box[4] = {64, (cuuint32_t)(box_w * sw), (cuuint32_t)(box_h * sh), (cuuint32_t)box_n};
     cuuint32_t estr[4] = {1, (cuuint32_t)sw, (cuuint32_t)sh, 1};
     if (box[1] > 256 || box[2] > 256) { set_cuda_error(cudaErrorInvalidValue, "conv tensor map: strided box too large"); return MR_ERR_UNSUPPORTED; }

@@ -288,36 +288,45 @@ def conv_fprop_tc(x, Wm, kh, kw, ph, pw, out_dtype=torch.bfloat16, bias=None, re
     return y, Ho, Wo
 
 
-def conv_fprop_pp(x, Wm, kh, kw, ph, pw):
-    """Persistent ping-pong implicit-GEMM conv (csrc/conv_pingpong.cu): x NHWC bf16 [N,H,W,C], Wm [Cout, kh*kw*C] bf16 ->
-    ([N*Ho*Wo, Cout] bf16, Ho, Wo), bit-identical to conv_fprop_tc's bf16 output.  None when the entry refuses the geometry
-    (MR_ERR_UNSUPPORTED): the caller then uses conv_fprop_tc."""
+def conv_fprop_pp(x, Wm, kh, kw, ph, pw, tile_m=0, out=None):
+    """Persistent implicit-GEMM conv (csrc/conv_pingpong.cu): x NHWC bf16 [N,H,W,C], Wm [Cout, kh*kw*C] bf16 -> ([N*Ho*Wo,
+    Cout] bf16, Ho, Wo), bit-identical to conv_fprop_tc's bf16 output.  Wm may be a column slice of a wider matrix.  `out`: an
+    [N, Ho, Wo, Cout] view to write instead, contiguous within an image (e.g. rows of a taller tensor); it is returned as
+    is.  tile_m: 128 / 256 force the 128- / 256-pixel-tile kernel, 0 lets the entry choose.  None when the entry refuses the
+    geometry (MR_ERR_UNSUPPORTED): the caller then uses conv_fprop_tc."""
     N, H, W, C = x.shape
     Cout = Wm.size(0)
-    assert x.is_contiguous() and Wm.is_contiguous() and Wm.size(1) == kh * kw * C
+    assert x.is_contiguous() and Wm.stride(1) == 1 and Wm.size(1) == kh * kw * C
     Ho, Wo = H + 2 * ph - kh + 1, W + 2 * pw - kw + 1
-    y = torch.empty((N * Ho * Wo, Cout), dtype=torch.bfloat16, device=x.device)
-    rc = _lib.lib().mr_conv_fprop_pp(_p(x), _p(Wm), _p(y), N, H, W, C, Cout, kh, kw, ph, pw, _st())
+    if out is None:
+        y, nstride = torch.empty((N * Ho * Wo, Cout), dtype=torch.bfloat16, device=x.device), 0
+    else:
+        assert out.shape == (N, Ho, Wo, Cout) and out.dtype == torch.bfloat16
+        assert out.stride()[1:] == (Wo * Cout, Cout, 1)
+        y, nstride = out, out.stride(0)
+    rc = _lib.lib().mr_conv_fprop_pp(_p(x), _p(Wm), _p(y), N, H, W, C, Cout, kh, kw, ph, pw, Wm.stride(0), nstride,
+                                     int(tile_m), _st())
     if rc == _lib.MR_ERR_UNSUPPORTED:
         return None
     _chk(rc, "conv_fprop_pp")
     return y, Ho, Wo
 
 
-def conv_wgrad_pp(dz, x, kh, kw, ph, pw, out=None):
+def conv_wgrad_pp(dz, x, kh, kw, ph, pw, out=None, ctas=None):
     """dWm [Cout, kh*kw*C] fp32 from dz [N,Ho,Wo,Cout] and x [N,H,W,C] (NHWC bf16) on the persistent 128 x 256 wgmma kernel
     (csrc/conv_pingpong.cu); `out`: a ZEROED [Cout, K] fp32 buffer to accumulate into.  None when the entry refuses the
-    geometry (MR_ERR_UNSUPPORTED): the caller then uses conv_wgrad_tc."""
+    geometry (MR_ERR_UNSUPPORTED): the caller then uses conv_wgrad_tc.  `ctas` caps the grid (default below)."""
     N, H, W, C = x.shape
     _, Ho, Wo, Cout = dz.shape
     K = kh * kw * C
     dWm = out if out is not None else torch.zeros((Cout, K), dtype=torch.float32, device=x.device)
-    # The kernel splits the K blocks of all 128 x 256 tiles evenly over its CTAs: one per SM, as long as each CTA still
-    # owns _WGRAD_MIN_KB K blocks to amortise the atomic flush of a tile.
-    rb = 80 if 64 < Wo <= 80 else 64
-    work = N * Ho * -(-Wo // rb) * -(-Cout // 128) * -(-K // 256)
-    ctas = min(torch.cuda.get_device_properties(x.device).multi_processor_count, max(1, work // _WGRAD_MIN_KB))
-    rc = _lib.lib().mr_conv_wgrad_pp(_p(dz), _p(x), _p(dWm), N, H, W, C, Cout, kh, kw, ph, pw, ctas, _st())
+    if ctas is None:
+        # One CTA per SM, as long as each CTA still owns _WGRAD_MIN_KB K blocks to amortise the atomic flush of a tile.
+        rb = 80 if 64 < Wo <= 80 else 64
+        work = N * Ho * -(-Wo // rb) * -(-Cout // 128) * -(-K // 256)
+        ctas = min(torch.cuda.get_device_properties(x.device).multi_processor_count, max(1, work // _WGRAD_MIN_KB))
+    rc = _lib.lib().mr_conv_wgrad_pp(_p(dz), _p(x), _p(dWm), N, H, W, C, Cout, kh, kw, ph, pw, int(ctas), _WGRAD_MIN_KB,
+                                     _st())
     if rc == _lib.MR_ERR_UNSUPPORTED:
         return None
     _chk(rc, "conv_wgrad_pp")
