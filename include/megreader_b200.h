@@ -225,6 +225,23 @@ int mr_db_batch(const void *images, int image_dtype, int64_t image_elems, const 
                 double *polygons_out, unsigned char *ignore_out, int *offsets_out, int *shape_out, int *crop_out, double *scale_out,
                 int *status, void *stream);
 
+/* Text crops for recognition (ImageCropper.crop; csrc/text_crop.cu) of every quad of N images.  images: one buffer of HWC
+ * pixels (image_dtype 0 = uint8, 1 = float32; image_elems elements), image n at element image_offsets[n] (device int64 [N]) with
+ * shapes[n] = (h, w) (device int32 [N, 2]).  quads (quad_dtype 0 = int32, 1 = float32): K > 0: [N, K, 4, 2] with count[n]
+ * quads of image n (count int32 [N]; quad_rows = N * K); K == 0: [quad_rows, 4, 2] with image n's at count[n] .. count[n + 1]
+ * (count int32 [N + 1]).  mode 0 "resize", 1 "pad".  Outputs, rows in (image, quad) order: image_out [capacity, 3, out_h,
+ * out_w] float32 (rows >= total untouched), owner [capacity, 2] int32 (image, quad; -1 past the total), total [1] (all quads,
+ * possibly more than capacity), status [N] (bits: 1 side outside 1..32766, 2 pixels outside the buffer, 4 count or offsets out
+ * of range -- such an image has no rows; 8 some quads beyond capacity; 16 a crop with int(w) or int(h) == 0 took the source's
+ * size; 32 a crop side above 32766, whose row is the zero canvas).  workspace >= mr_text_crop_workspace_bytes(N, capacity).
+ * MR_ERR_BAD_SHAPE for N outside 1..65535, capacity outside 0..65535, bad dtypes or mode, an empty output size, or a smaller
+ * workspace, before any CUDA call.  No host synchronisation: the call can be captured in a CUDA graph. */
+int64_t mr_text_crop_workspace_bytes(int64_t N, int64_t capacity);
+int mr_text_crop(const void *images, int image_dtype, int64_t image_elems, const int64_t *image_offsets, const int *shapes, int N,
+                 const void *quads, int quad_dtype, int64_t quad_rows, int K, const int *count, int capacity, int mode, int out_h,
+                 int out_w, double mean0, double mean1, double mean2, void *workspace, int64_t workspace_bytes, float *image_out,
+                 int *owner, int *total, int *status, void *stream);
+
 int64_t mr_db_measure_workspace_bytes(int64_t N, int64_t capacity, int64_t max_dets);
 int mr_db_measure(const void *gt_polygons, int gt_dtype, const unsigned char *ignore_tags, const int *offsets, int N, int capacity,
                   const void *boxes, int det_dtype, const int *count, int max_dets, double iou_constraint,

@@ -71,21 +71,56 @@ __host__ __device__ inline int trace_border(const unsigned char *bm, int H, int 
 
 }  // namespace mr_dbbox
 
+namespace mr_dbbox {
+
+// float products and sums that must round exactly as cv2's x86 build (no fused multiply-add) does
+#ifdef __CUDA_ARCH__
+__device__ __forceinline__ float fmul(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float fadd(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ float fsub(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
+#else
+inline float fmul(float a, float b) { return a * b; }
+inline float fadd(float a, float b) { return a + b; }
+inline float fsub(float a, float b) { return a - b; }
+inline double dmul(double a, double b) { return a * b; }
+inline double dadd(double a, double b) { return a + b; }
+inline double dsub(double a, double b) { return a - b; }
+#endif
+
+}  // namespace mr_dbbox
+
 // ---- per-candidate geometry (seg_detector_representer.py:81-85, 125-145: get_mini_boxes = cv2.minAreaRect + cv2.boxPoints) ----
 namespace mr_dbbox {
 
-struct Pt { int x, y; };
+// A point of cv::convexHull's input: int (contours) or float (cv2.minAreaRect of float32 polygons)
+template <class T> struct PtT { T x, y; };
+using Pt = PtT<int>;
 
+__host__ __device__ inline int sgn(int v) { return (v > 0) - (v < 0); }
 __host__ __device__ inline int sgn(int64_t v) { return (v > 0) - (v < 0); }
+__host__ __device__ inline int sgn(double v) { return (v > 0) - (v < 0); }
 
-__host__ __device__ inline bool pt_less(const Pt *p, int a, int b) {
+// Sklansky's coordinate differences and convexity: int with an int64 cross product, or float with a double one
+__host__ __device__ inline int hull_sub(int a, int b) { return a - b; }
+__host__ __device__ inline float hull_sub(float a, float b) { return fsub(a, b); }
+__host__ __device__ inline int64_t hull_cross(int ay, int bx, int ax, int by) { return (int64_t)ay * bx - (int64_t)ax * by; }
+__host__ __device__ inline double hull_cross(float ay, float bx, float ax, float by) {
+    return dsub(dmul((double)ay, (double)bx), dmul((double)ax, (double)by));
+}
+
+template <class T>
+__host__ __device__ inline bool pt_less(const PtT<T> *p, int a, int b) {
     return p[a].x < p[b].x || (p[a].x == p[b].x && p[a].y < p[b].y);
 }
 
 // std::sort as libstdc++ implements it (median-of-three quicksort down to runs of 16, heap sort past 2 log2(n) levels, then one
 // insertion sort) of the indices idx[0..n) by (x, y), the order cv::convexHull sorts its point pointers in.  The comparison
 // does not separate equal points; which of them cv2 ends up reporting is not always this sort's choice (see convex_hull).
-__host__ __device__ inline void sift_down(const Pt *p, int *a, int hole, int len, int value) {
+template <class T>
+__host__ __device__ inline void sift_down(const PtT<T> *p, int *a, int hole, int len, int value) {
     const int top = hole;
     int child = hole;
     while (child < (len - 1) / 2) {
@@ -108,7 +143,8 @@ __host__ __device__ inline void sift_down(const Pt *p, int *a, int hole, int len
     a[hole] = value;
 }
 
-__host__ __device__ inline void heap_sort(const Pt *p, int *a, int len) {
+template <class T>
+__host__ __device__ inline void heap_sort(const PtT<T> *p, int *a, int len) {
     if (len < 2) return;
     for (int parent = (len - 2) / 2;; --parent) {
         sift_down(p, a, parent, len, a[parent]);
@@ -123,7 +159,8 @@ __host__ __device__ inline void heap_sort(const Pt *p, int *a, int len) {
 
 __host__ __device__ inline void swap_idx(int *a, int i, int j) { const int t = a[i]; a[i] = a[j]; a[j] = t; }
 
-__host__ __device__ inline void sort_points(const Pt *p, int *a, int n) {
+template <class T>
+__host__ __device__ inline void sort_points(const PtT<T> *p, int *a, int n) {
     if (n < 2) return;
     int lg = 0;
     while ((2 << lg) <= n) ++lg;
@@ -181,7 +218,8 @@ __host__ __device__ inline void sort_points(const Pt *p, int *a, int n) {
 }
 
 // one monotone chain of cv::convexHull's Sklansky scan over the sorted order
-__host__ __device__ inline int sklansky(const Pt *p, const int *o, int start, int end, int *stack, int nsign, int sign2) {
+template <class T>
+__host__ __device__ inline int sklansky(const PtT<T> *p, const int *o, int start, int end, int *stack, int nsign, int sign2) {
     const int incr = end > start ? 1 : -1;
     int pprev = start, pcur = pprev + incr, pnext = pcur + incr;
     int stacksize = 3;
@@ -194,11 +232,11 @@ __host__ __device__ inline int sklansky(const Pt *p, const int *o, int start, in
     stack[2] = pnext;
     end += incr;
     while (pnext != end) {
-        const int cury = p[o[pcur]].y, nexty = p[o[pnext]].y, by = nexty - cury;
+        const T cury = p[o[pcur]].y, nexty = p[o[pnext]].y, by = hull_sub(nexty, cury);
         if (sgn(by) != nsign) {
-            const int ax = p[o[pcur]].x - p[o[pprev]].x, bx = p[o[pnext]].x - p[o[pcur]].x, ay = cury - p[o[pprev]].y;
-            const int64_t convexity = (int64_t)ay * bx - (int64_t)ax * by;
-            if (sgn(convexity) == sign2 && (ax != 0 || ay != 0)) {
+            const T ax = hull_sub(p[o[pcur]].x, p[o[pprev]].x), bx = hull_sub(p[o[pnext]].x, p[o[pcur]].x);
+            const T ay = hull_sub(cury, p[o[pprev]].y);
+            if (sgn(hull_cross(ay, bx, ax, by)) == sign2 && (ax != 0 || ay != 0)) {
                 pprev = pcur;
                 pcur = pnext;
                 pnext += incr;
@@ -227,12 +265,13 @@ __host__ __device__ inline int sklansky(const Pt *p, const int *o, int start, in
 // cyclic order are cv2's; where a vertex occurs more than once in p, cv2 may report another of its copies and therefore start
 // the (index-ordered) hull elsewhere (~0.5 % of contours, tests/test_db_boxes_cpu.py).  Scratch: o[n], stack[n + 2].  Returns the
 // number of hull vertices.
-__host__ __device__ inline int convex_hull(const Pt *p, int n, int *o, int *stack, int *hull) {
+template <class T>
+__host__ __device__ inline int convex_hull(const PtT<T> *p, int n, int *o, int *stack, int *hull) {
     for (int i = 0; i < n; ++i) o[i] = i;
     sort_points(p, o, n);
     int miny = 0, maxy = 0;
     for (int i = 1; i < n; ++i) {
-        const int y = p[o[i]].y;
+        const T y = p[o[i]].y;
         if (p[o[miny]].y > y) miny = i;
         if (p[o[maxy]].y < y) maxy = i;
     }
@@ -300,23 +339,6 @@ __host__ __device__ inline int convex_hull(const Pt *p, int n, int *o, int *stac
 
 namespace mr_dbbox {
 
-// float products and sums that must round exactly as cv2's x86 build (no fused multiply-add) does
-#ifdef __CUDA_ARCH__
-__device__ __forceinline__ float fmul(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ float fadd(float a, float b) { return __fadd_rn(a, b); }
-__device__ __forceinline__ float fsub(float a, float b) { return __fsub_rn(a, b); }
-__device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
-#else
-inline float fmul(float a, float b) { return a * b; }
-inline float fadd(float a, float b) { return a + b; }
-inline float fsub(float a, float b) { return a - b; }
-inline double dmul(double a, double b) { return a * b; }
-inline double dadd(double a, double b) { return a + b; }
-inline double dsub(double a, double b) { return a - b; }
-#endif
-
 struct Rect { float cx, cy, w, h, angle; };
 
 __host__ __device__ inline float degrees(double rad) { return (float)(dmul(rad, 180.) / 3.14159265358979323846); }
@@ -335,7 +357,8 @@ __host__ __device__ inline Rect min_area_rect_hull(const float *qx, const float 
             if (py0 > top_y) { top_y = py0; top = i; }
             if (py0 < bottom_y) { bottom_y = py0; bottom = i; }
             const int j = i + 1 < n ? i + 1 : 0;
-            const double dx = dsub((double)qx[j], (double)px0), dy = dsub((double)qy[j], (double)py0);
+            // float differences (exact for the integer points of contours), then double as cv2 has them
+            const double dx = fsub(qx[j], px0), dy = fsub(qy[j], py0);
             vx[i] = (float)dx;
             vy[i] = (float)dy;
             inv[i] = (float)(1. / sqrt(dadd(dmul(dx, dx), dmul(dy, dy))));
@@ -444,13 +467,10 @@ __host__ __device__ inline Rect min_area_rect_hull(const float *qx, const float 
 
 namespace mr_dbbox {
 
-// cv2.boxPoints(rect) followed by get_mini_boxes' ordering (seg_detector_representer.py:125-145): the corners sorted by x
-// (a stable sort), then of the two left ones the lower-y first, of the two right ones the lower-y second.  box[8] = (x, y) x 4.
-// Returns min(width, height) ("sside").
-__host__ __device__ inline float mini_box(const Rect &r, float *box) {
+// cv2.boxPoints(rect): px[4], py[4]
+__host__ __device__ inline void box_points(const Rect &r, float *px, float *py) {
     const double ang = (double)r.angle * 3.14159265358979323846 / 180.;
     const float b = fmul((float)cos(ang), 0.5f), a = fmul((float)sin(ang), 0.5f);
-    float px[4], py[4];
     px[0] = fsub(fsub(r.cx, fmul(a, r.h)), fmul(b, r.w));
     py[0] = fsub(fadd(r.cy, fmul(b, r.h)), fmul(a, r.w));
     px[1] = fsub(fadd(r.cx, fmul(a, r.h)), fmul(b, r.w));
@@ -459,6 +479,14 @@ __host__ __device__ inline float mini_box(const Rect &r, float *box) {
     py[2] = fsub(fmul(2.f, r.cy), py[0]);
     px[3] = fsub(fmul(2.f, r.cx), px[1]);
     py[3] = fsub(fmul(2.f, r.cy), py[1]);
+}
+
+// cv2.boxPoints(rect) followed by get_mini_boxes' ordering (seg_detector_representer.py:125-145): the corners sorted by x
+// (a stable sort), then of the two left ones the lower-y first, of the two right ones the lower-y second.  box[8] = (x, y) x 4.
+// Returns min(width, height) ("sside").
+__host__ __device__ inline float mini_box(const Rect &r, float *box) {
+    float px[4], py[4];
+    box_points(r, px, py);
     int o[4] = {0, 1, 2, 3};
     for (int i = 1; i < 4; ++i)                       // stable insertion sort by x
         for (int j = i; j > 0 && px[o[j]] < px[o[j - 1]]; --j) { const int t = o[j]; o[j] = o[j - 1]; o[j - 1] = t; }
