@@ -624,6 +624,22 @@ int mr_attn_train_bwd_f32(const float *projected, const float *memory, const flo
                           int E, int V, int S, void *stream);
 int mr_attn_sync_status(const void *sync, void *stream, int *status);
 
+/* Baseline JPEG decoding (csrc/jpeg.cu) of N images, each equal to cv2.imdecode(buf, cv2.IMREAD_COLOR).  data: the packed
+ * bytes (device, data_bytes), image n's at data_offsets[n] .. data_offsets[n + 1] (device int64 [N + 1], non-decreasing;
+ * an image whose bytes start inside an earlier image's is flagged 32).
+ * Outputs in db_batch's packed layout: image_out uint8 HWC BGR (3 * pixel_capacity bytes), image_offsets int64 [N] (elements,
+ * a prefix sum over the images), shapes int32 [N, 2] (h, w after the EXIF orientation), status int32 [N] (bits: 1 not a JPEG
+ * or a malformed header; 2 an unsupported process -- progressive, arithmetic, lossless, hierarchical, 12-bit, DNL, or a frame
+ * in more than one scan; 4 unsupported components -- 2 or 4 components, fractional sampling; 8 a side above max_h / max_w, or
+ * beyond the pixel or coefficient capacity; 16 corrupt entropy-coded data; 32 offsets outside the buffer).  A flagged image
+ * has shape (0, 0) and no pixels.  workspace >= mr_jpeg_workspace_bytes(N, data_bytes, pixel_capacity).  MR_ERR_BAD_SHAPE
+ * for N outside 1..65535, max_h or max_w outside 1..16384, or a smaller workspace, before any CUDA call.  No host
+ * synchronisation and no allocation: the call can be captured in a CUDA graph. */
+int64_t mr_jpeg_workspace_bytes(int64_t N, int64_t byte_capacity, int64_t pixel_capacity);
+int mr_jpeg_decode(const void *data, int64_t data_bytes, const int64_t *data_offsets, int N, int max_h, int max_w, int64_t pixel_capacity,
+                   void *workspace, int64_t workspace_bytes, unsigned char *image_out, int64_t *image_offsets, int *shapes, int *status,
+                   void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -118,6 +118,8 @@ _SIGS = {
     "mr_text_crop_workspace_bytes": [c_i64, c_i64],
     "mr_text_crop": [c_p, c_int, c_i64, c_p, c_p, c_int, c_p, c_int, c_i64, c_int, c_p, c_int, c_int, c_int, c_int]
                     + [ctypes.c_double] * 3 + [c_p, c_i64] + [c_p] * 5,
+    "mr_jpeg_workspace_bytes": [c_i64] * 3,
+    "mr_jpeg_decode": [c_p, c_i64, c_p, c_int, c_int, c_int, c_i64, c_p, c_i64, c_p, c_p, c_p, c_p, c_p],
     "mr_rec_lexicon_build_bytes": [c_i64],
     "mr_rec_lexicon_build": [c_p, c_p, c_int, c_p, c_i64, c_p],
     "mr_rec_measure_workspace_bytes": [c_i64, c_i64, c_i64, c_int],
@@ -134,6 +136,7 @@ _RESTYPES = {
     "mr_rec_measure_workspace_bytes": c_i64,
     "mr_db_batch_workspace_bytes": c_i64,
     "mr_text_crop_workspace_bytes": c_i64,
+    "mr_jpeg_workspace_bytes": c_i64,
     "mr_db_loss_workspace_bytes": c_i64,
     "mr_dcn_fused_workspace_bytes_h": c_i64,
     "mr_dcn_fused_backward_workspace_bytes_h": c_i64,

@@ -62,6 +62,40 @@ def resize_normalize(images, image_size, mode="resize", device=None, mean=RGB_ME
     return out
 
 
+def resize_normalize_packed(buffer, image_offsets, shapes, image_size, mode="resize", mean=RGB_MEAN):
+    """resize_normalize of images already on the device in db_batch's packed layout (HWC uint8, as jpeg.decode_packed
+    returns them): float32 [N, 3, H, W].  resized_width is computed on the device in float64 with the same expression, so
+    there is no host read.  Rows of images with shape (0, 0) are zero."""
+    for name, t in (("buffer", buffer), ("image_offsets", image_offsets), ("shapes", shapes)):
+        if not (torch.is_tensor(t) and t.is_cuda):
+            raise NotImplementedError("megreader_b200: the input step runs on CUDA only (no CPU fallback); %s is not a CUDA tensor" % name)
+    if buffer.dtype != torch.uint8 or image_offsets.dtype != torch.int64 or shapes.dtype != torch.int32 or shapes.dim() != 2:
+        raise RuntimeError("resize_normalize_packed: expected uint8 buffer, int64 image_offsets and int32 shapes [N, 2]")
+    n = shapes.size(0)
+    dst_h, dst_w = int(image_size[0]), int(image_size[1])
+    out = torch.empty((n, 3, dst_h, dst_w), dtype=torch.float32, device=buffer.device)
+    if n == 0:
+        return out
+    ok = shapes[:, 0] > 0
+    hs = torch.where(ok, shapes[:, 0], 1).contiguous()
+    ws = torch.where(ok, shapes[:, 1], 1).contiguous()
+    offs = torch.where(ok, image_offsets, 0).contiguous()
+    if mode == "pad":
+        v = torch.trunc(dst_h / hs.double() * ws.double() / 32 + 0.5) * 32
+        valid = torch.clamp(v, min=32, max=dst_w).to(torch.int32)
+    elif mode == "resize":
+        valid = torch.full_like(hs, dst_w)
+    else:
+        raise ValueError("batched input step supports modes 'resize' and 'pad' (fixed-size outputs), got %r" % (mode,))
+    mean3 = (ctypes.c_double * 3)(*mean)
+    with torch.cuda.device(buffer.device):
+        _lib.check(_lib.lib().mr_resize_normalize_f32(buffer.data_ptr(), 1, offs.data_ptr(), hs.data_ptr(), ws.data_ptr(),
+                                                      valid.data_ptr(), n, dst_h, dst_w, ctypes.cast(mean3, ctypes.c_void_p),
+                                                      out.data_ptr(), _stream()),
+                   "resize_normalize_packed")
+    return out.mul_(ok.view(n, 1, 1, 1))
+
+
 def charset_lut(charset=None):
     """256-entry byte -> class-index table of a charset (`Charset.index`, concern/charsets.py: unknown for anything else)."""
     charset = charset if charset is not None else default_charset()
