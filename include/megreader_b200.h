@@ -517,7 +517,7 @@ int mr_lstm_step_bwd_tcgen05(const void *const *dG_next, const void *const *Whh,
  *   G     : [2, T, B, 4H] bf16 -- x-projection on entry, activated gates (i,f,g,o) on exit
  *   bias  : HOST array of 2 device pointers, [4H] fp32 unit-major (b_ih + b_hh)
  *   C     : [2, T, B, H] fp32 cell states, out;   Y : [T, B, 2H] bf16 layer output, out (direction d -> columns d*H..)
- *   flags : [2*ceil(B/128) + 1] uint32 scratch (zeroed by the call); after completion the last word is 0, or a non-zero
+ *   flags : [2*ceil(B/64) + 1] uint32 scratch (zeroed by the call); after completion the last word is 0, or a non-zero
  *           code if an inter-CTA wait timed out (results then undefined)
  * bwd:  dY [T, B, 2H] bf16 -> dG [2, T, B, 4H] bf16 gate gradients (the weight/input gradients are plain GEMMs on dG);
  *       WhhT = the recurrent weights TRANSPOSED, HOST array of 2 device pointers to [H, 4H] bf16 (unit-major columns).

@@ -398,7 +398,9 @@ def lstm_step_bwd_tc(dG_next, Whh, gates, c, c_prev, dh_out, ldh, dc, dgates, ha
 
 
 def lstm_seq_flags(B, device):
-    return torch.empty((2 * ((B + 127) // 128) + 1,), dtype=torch.int32, device=device)
+    """Scratch of the persistent recurrence: arrival counters per direction and 64-row tile (the backward's tiling, the
+    finer of the two), then the error word."""
+    return torch.empty((2 * ((B + 63) // 64) + 1,), dtype=torch.int32, device=device)
 
 
 def lstm_seq_fwd_tc(Whh, G, bias, C, Y, flags):
