@@ -640,6 +640,30 @@ int mr_jpeg_decode(const void *data, int64_t data_bytes, const int64_t *data_off
                    void *workspace, int64_t workspace_bytes, unsigned char *image_out, int64_t *image_offsets, int *shapes, int *status,
                    void *stream);
 
+/* PNG decoding (csrc/png.cu) of N images, each equal to cv2.imdecode(buf, cv2.IMREAD_COLOR): every colour type and bit depth,
+ * Adam7, the eXIf orientation; 16-bit samples reduced to their high byte, alpha and tRNS dropped.  The arguments, the output
+ * layout and the capacity rule are mr_jpeg_decode's.  Status bits: 1 not a PNG, a malformed IHDR or chunk structure, a CRC
+ * error in IHDR, PLTE or IDAT, IDAT chunks interrupted before the image data ends, no IEND, no PLTE for colour type 3; 2 an
+ * APNG whose IDAT image is not its first frame; 8 a side above max_h / max_w or 16384, or beyond the pixel capacity; 16
+ * corrupt compressed data (a bad zlib header, an invalid deflate stream, data that ends early, a wrong Adler-32, a row
+ * filter past 4); 32 offsets outside the buffer.  A flagged image has shape (0, 0) and no pixels.
+ * workspace >= mr_png_workspace_bytes(N, data_bytes, pixel_capacity), about data_bytes + 69 * pixel_capacity: the gathered
+ * zlib streams, the inflated rows (at most 9 bytes per pixel), a 4-byte copy source per inflated byte and the match records.
+ * MR_ERR_BAD_SHAPE as mr_jpeg_decode's, before any CUDA call.  No host synchronisation and no allocation. */
+int64_t mr_png_workspace_bytes(int64_t N, int64_t byte_capacity, int64_t pixel_capacity);
+int mr_png_decode(const void *data, int64_t data_bytes, const int64_t *data_offsets, int N, int max_h, int max_w, int64_t pixel_capacity,
+                  void *workspace, int64_t workspace_bytes, unsigned char *image_out, int64_t *image_offsets, int *shapes, int *status,
+                  void *stream);
+/* Decoding of N images that may each be JPEG or PNG (the replacement of cv2.imread / cv2.imdecode(buf, cv2.IMREAD_COLOR)):
+ * each image by the decoder whose signature it carries, a file with neither flagged 1.  Every JPEG comes out as
+ * mr_jpeg_decode decodes it, every PNG as mr_png_decode does; the capacity rule applies to the merged pixel sums.  Arguments
+ * and outputs as mr_jpeg_decode's.  workspace >= mr_image_workspace_bytes(N, data_bytes, pixel_capacity): the larger of
+ * the two decoders' workspaces, which run one after the other, plus 2 * 3 * pixel_capacity bytes for their pixels. */
+int64_t mr_image_workspace_bytes(int64_t N, int64_t byte_capacity, int64_t pixel_capacity);
+int mr_image_decode(const void *data, int64_t data_bytes, const int64_t *data_offsets, int N, int max_h, int max_w, int64_t pixel_capacity,
+                    void *workspace, int64_t workspace_bytes, unsigned char *image_out, int64_t *image_offsets, int *shapes, int *status,
+                    void *stream);
+
 #ifdef __cplusplus
 }
 #endif

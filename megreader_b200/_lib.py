@@ -120,6 +120,10 @@ _SIGS = {
                     + [ctypes.c_double] * 3 + [c_p, c_i64] + [c_p] * 5,
     "mr_jpeg_workspace_bytes": [c_i64] * 3,
     "mr_jpeg_decode": [c_p, c_i64, c_p, c_int, c_int, c_int, c_i64, c_p, c_i64, c_p, c_p, c_p, c_p, c_p],
+    "mr_png_workspace_bytes": [c_i64] * 3,
+    "mr_png_decode": [c_p, c_i64, c_p, c_int, c_int, c_int, c_i64, c_p, c_i64, c_p, c_p, c_p, c_p, c_p],
+    "mr_image_workspace_bytes": [c_i64] * 3,
+    "mr_image_decode": [c_p, c_i64, c_p, c_int, c_int, c_int, c_i64, c_p, c_i64, c_p, c_p, c_p, c_p, c_p],
     "mr_rec_lexicon_build_bytes": [c_i64],
     "mr_rec_lexicon_build": [c_p, c_p, c_int, c_p, c_i64, c_p],
     "mr_rec_measure_workspace_bytes": [c_i64, c_i64, c_i64, c_int],
@@ -137,6 +141,8 @@ _RESTYPES = {
     "mr_db_batch_workspace_bytes": c_i64,
     "mr_text_crop_workspace_bytes": c_i64,
     "mr_jpeg_workspace_bytes": c_i64,
+    "mr_png_workspace_bytes": c_i64,
+    "mr_image_workspace_bytes": c_i64,
     "mr_db_loss_workspace_bytes": c_i64,
     "mr_dcn_fused_workspace_bytes_h": c_i64,
     "mr_dcn_fused_backward_workspace_bytes_h": c_i64,

@@ -123,11 +123,10 @@ __host__ __device__ inline bool make_huff(const uint8_t bits[17], const uint8_t 
     return true;
 }
 
-// OpenCV's EXIF orientation: IFD0 tag 0x0112 of the first APP1 "Exif\0\0" segment, either TIFF byte order; 1 when absent
-__host__ __device__ inline int exif_orientation(const uint8_t *d, int64_t n) {
-    if (n < 14 || d[0] != 'E' || d[1] != 'x' || d[2] != 'i' || d[3] != 'f' || d[4] != 0 || d[5] != 0) return 1;
-    const uint8_t *t = d + 6;
-    const int64_t tn = n - 6;
+// OpenCV's EXIF orientation from TIFF data t[0, tn) (a JPEG APP1 payload after "Exif\0\0", or a PNG eXIf chunk): IFD0 tag
+// 0x0112, either byte order; 1 when absent
+__host__ __device__ inline int tiff_orientation(const uint8_t *t, int64_t tn) {
+    if (tn < 8) return 1;
     bool le;
     if (t[0] == 'I' && t[1] == 'I') le = true;
     else if (t[0] == 'M' && t[1] == 'M') le = false;
@@ -150,6 +149,12 @@ __host__ __device__ inline int exif_orientation(const uint8_t *d, int64_t n) {
         }
     }
     return 1;
+}
+
+// the first APP1 "Exif\0\0" segment's orientation
+__host__ __device__ inline int exif_orientation(const uint8_t *d, int64_t n) {
+    if (n < 14 || d[0] != 'E' || d[1] != 'x' || d[2] != 'i' || d[3] != 'f' || d[4] != 0 || d[5] != 0) return 1;
+    return tiff_orientation(d + 6, n - 6);
 }
 
 __host__ __device__ inline int ceil_div_i(int a, int b) { return (a + b - 1) / b; }
