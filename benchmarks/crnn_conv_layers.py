@@ -16,7 +16,8 @@ bf16 NHWC activations).
     gradient on the 128-pixel ping-pong kernel (tile_m=128) and as mr_conv_fprop_pp selects (tile_m=0: the 256-pixel
     kernel from 36 K blocks on), L6's input gradient also as the engine's row split (two 1 x 2 convolutions), and the
     weight gradient with the planner's schedule (its old arm is this script's (a) run from the parent build).  Beside
-    TFLOP/s it prints the L2-to-SM rate implied by the kernel's operand bytes per FLOP.
+    TFLOP/s it prints the L2-to-SM rate implied by the kernel's operand bytes per FLOP, and for the weight gradient the
+    share of the issued MMA work that multiplies real pixels and columns rather than zero fill.
         python benchmarks/crnn_conv_layers.py --changed --out DIR [--batch 512] [--rounds 3]
 
 All write JSON into DIR together with the card's name, power limit and maximum SM clock.  L0 (Cin = 3) runs on the fused
@@ -144,8 +145,18 @@ def changed_calls(n, dev):
     return out
 
 
+def wgrad_useful_mma(name, n, sms):
+    """Share of the weight gradient's issued MMA work that multiplies real operands: the useful products over the K blocks
+    (RB pixels each, zero fill included) x 128 x 256 tiles of mr_conv_wgrad_pp's plan."""
+    _, H, W, C, Cout, k, p = next(lay for lay in LAYERS if lay[0] == name)
+    Ho, Wo = H + 2 * p - k + 1, W + 2 * p - k + 1
+    plan = ops.conv_wgrad_pp_plan(n, H, W, C, Cout, k, k, p, p, sms)
+    return n * Ho * Wo * Cout * k * k * C / (plan["kb_total"] * plan["RB"] * plan["tiles"] * 128 * 256)
+
+
 def run_changed(args):
     dev = torch.device("cuda:0")
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
     cs = changed_calls(args.batch, dev)
     times = defaultdict(list)
     for _ in range(args.rounds):
@@ -165,12 +176,15 @@ def run_changed(args):
                 r = fn()
                 ref = r.clone() if ref is None else ref
                 row[arm]["same_bits_as_pp128"] = bool(torch.equal(r.view_as(ref), ref))
+        if kind == "wgrad":
+            row["useful_mma"] = wgrad_useful_mma(name, args.batch, sms)
         rows.append(row)
         print("%-3s %-6s %s" % (name, kind, "  ".join(
             "%s %7.1f us (%s) %6.1f TFLOP/s L2 %4.1f TB/s%s" % (
                 arm, v["us"], "/".join("%.0f" % u for u in v["us_all"]), v["tflops"], v["l2_tb_s"],
                 "" if v.get("same_bits_as_pp128", True) else " DIFFERENT")
-            for arm, v in row.items() if isinstance(v, dict))), flush=True)
+            for arm, v in row.items() if isinstance(v, dict)) +
+            ("  useful MMA %.1f %% of issued" % (100 * row["useful_mma"]) if kind == "wgrad" else "")), flush=True)
     return {"batch": args.batch, "iters_per_graph": args.iters, "rounds": args.rounds, "calls": rows}
 
 

@@ -496,6 +496,15 @@ int mr_conv_fprop_pp(const void *x, const void *Wm, void *y, int N, int H, int W
  * uses mr_conv_wgrad_tcgen05). */
 int mr_conv_wgrad_pp(const void *dz, const void *x, float *dWm, int N, int H, int W, int C, int Cout, int kh, int kw, int ph,
                      int pw, int ctas, int min_kb, void *stream);
+/* Host only, no device needed: the schedule mr_conv_wgrad_pp runs on `ctas` (>= 1) CTAs with `min_kb`, written to
+ * plan[MR_WGRAD_PP_PLAN_INTS] as {RB, grid, kb_total, tiles, kb_split, units, balanced, nseg} followed by five segments
+ * (w0, bw, bn, w_blocks, kb_begin), unused ones zero.  A K block is RB output pixels: a box of bw columns x 1 row x bn
+ * images at column w0 + bw * (i % w_blocks), row i / w_blocks % Ho, images bn * (i / w_blocks / Ho) for the segment's
+ * i-th block, kb_begin + i.  The (split, tile) units, `units` of them with kb_split K blocks per split, are dealt to `grid`
+ * CTAs; balanced = 1: every CTA gets the same number. */
+#define MR_WGRAD_PP_PLAN_INTS 33
+int mr_conv_wgrad_pp_plan(int N, int H, int W, int C, int Cout, int kh, int kw, int ph, int pw, int ctas, int min_kb,
+                          int *plan);
 
 /* Fused LSTM time steps on wgmma (recurrent GEMM + cell in one launch, both directions): gate columns are
  * UNIT-MAJOR (column 4*j + g = gate g in {i,f,g,o} of hidden unit j), H % 64 == 0, bf16.  Every per-direction argument

@@ -351,20 +351,57 @@ conv_fprop_m256_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_con
 //
 // CTA tile 128 (Cout) x 256 (kh*kw*C columns): both consumer warpgroups read the same dz (A) stage and each owns one
 // 128-column half of the x (B) operand, so a stage of dz is loaded once per 256 columns.  Both operands come MN-major by
-// 4-D TMA exactly as in conv_wgrad_tcgen05_kernel (K block = RB output pixels of one row; tap shift = signed coordinate
-// offset, padding = TMA zero fill).  The K blocks are cut into `splits` equal splits; a unit is one (split, tile), and the
-// units, numbered split-major, are handed out strided by gridDim.x.  The planner makes the unit count a whole multiple of
-// the grid, so every CTA gets the same number of units, and the CTAs that run side by side work on one split or on
-// adjacent ones, i.e. on the same rows of dz and x, which are then read from HBM once and hit in L2 by the other tiles.  A
-// CTA accumulates a unit in registers and adds it into dW (pre-zeroed by the caller) straight from the fragments with
-// red.global.add.v4.f32.
+// 4-D TMA (tap shift = signed coordinate offset, padding = TMA zero fill).  A K block is RB output pixels, the box
+// bw columns x 1 row x bn images (bw * bn = RB) of one segment of the plan_wgrad_segments plan; dz and x are loaded with
+// boxes of the same geometry, so row r of both operand tiles is the same output pixel and the order of the pixels does not
+// matter.  The segments tile the output width exactly, so only a segment's last image block multiplies zero fill.  The K
+// blocks are cut into `splits` equal splits; a unit is one (split, tile), and the units, numbered split-major, are handed
+// out strided by gridDim.x.  The planner makes the unit count a whole multiple of the grid, so every CTA gets the same
+// number of units, and the CTAs that run side by side work on one split or on adjacent ones, i.e. on the same images of dz
+// and x, which are then read from HBM once and hit in L2 by the other tiles.  A CTA accumulates a unit in registers and
+// adds it into dW (pre-zeroed by the caller) straight from the fragments with red.global.add.v4.f32.
 // =====================================================================================================
+// K-block segments of the weight gradient: columns [w0, w0 + w_blocks * bw) of the output, in boxes of bw x 1 x bn
+// pixels; the segment's K blocks are numbered from kb_begin, box column fastest, then the output row, then the image block.
+constexpr int kMaxWgradSegs = 5;
+struct WgradSeg { int w0, bw, bn, w_blocks, kb_begin; };
+
 struct PpWgradArgs {
-    int C, Cout, K, kw, ph, pw, Ho, wboxes;
+    int C, Cout, K, kw, ph, pw, Ho;
+    int nseg;
+    WgradSeg seg[kMaxWgradSegs];
     int kb_total, n_tiles, tiles;     // K blocks per tile; 256-column tiles per 128-row block; all tiles
     int kb_split;                     // K blocks per split (the last split may be shorter, or empty)
     int units;                        // splits x tiles
 };
+// One dz and one x tensor map per segment, with that segment's box.
+struct WgradMaps { CUtensorMap dz[kMaxWgradSegs], x[kMaxWgradSegs]; };
+
+// Output pixels per K block: 80 when 64 < Wo <= 80 (L4-L6 of the CRNN, Wo = 65 and 66), 64 otherwise.
+__host__ __device__ constexpr int wgrad_rb(int Wo) { return Wo > 64 && Wo <= 80 ? 80 : 64; }
+
+// The K-block segments of an [N, Ho, Wo] output.  RB = 80: the first floor(Wo / 16) * 16 columns in 16 x 1 x 5 boxes,
+// then the rest in power-of-two widths bw = 8, 4, 2, 1, each in bw x 1 x (80 / bw) boxes (Wo = 65: 1,676 K blocks at
+// L5 instead of the 2,048 of one 80-wide box per row, 99.3 % of them real pixels).  RB = 64: one segment of RB-wide row
+// boxes.  -> the K-block total.
+int64_t plan_wgrad_segments(int N, int Ho, int Wo, int RB, WgradSeg *seg, int *nseg) {
+    int64_t kb = 0;
+    *nseg = 0;
+    auto add = [&](int w0, int bw, int w_blocks) {
+        WgradSeg &s = seg[(*nseg)++];
+        s.w0 = w0; s.bw = bw; s.bn = RB / bw; s.w_blocks = w_blocks; s.kb_begin = (int)kb;
+        kb += (int64_t)w_blocks * Ho * ceil_div(N, s.bn);
+    };
+    if (RB == 80) {
+        const int w16 = Wo / 16 * 16;
+        add(0, 16, Wo / 16);
+        for (int bw = 8, w0 = w16; bw >= 1; bw >>= 1)
+            if ((Wo - w16) & bw) { add(w0, bw, 1); w0 += bw; }
+    } else {
+        add(0, RB, (int)ceil_div(Wo, RB));
+    }
+    return kb;
+}
 
 // Unit u = (split u / tiles, tile u % tiles): K blocks [kb_lo, kb_hi) of `tile`.
 struct WgradUnit { int tile, kb_lo, kb_hi; };
@@ -391,8 +428,7 @@ __device__ __forceinline__ void red_add_v4(float *p, float a, float b, float c, 
 
 template <int RB>
 __global__ void __launch_bounds__(kPpThreads, 1)
-conv_wgrad_pp_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_constant__ CUtensorMap tmX,
-                     float *__restrict__ dW, const __grid_constant__ PpWgradArgs a) {
+conv_wgrad_pp_kernel(const __grid_constant__ WgradMaps tm, float *__restrict__ dW, const __grid_constant__ PpWgradArgs a) {
     using L = PpWgradSmem<RB>;
     constexpr int STAGES = L::STAGES;
     extern __shared__ unsigned char smem_raw[];
@@ -402,8 +438,7 @@ conv_wgrad_pp_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_cons
     const int wg = threadIdx.x >> 7;
 
     if (threadIdx.x == 0) {
-        tma_prefetch_desc(&tmDz);
-        tma_prefetch_desc(&tmX);
+        for (int q = 0; q < a.nseg; ++q) { tma_prefetch_desc(&tm.dz[q]); tma_prefetch_desc(&tm.x[q]); }
         for (int s = 0; s < STAGES; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 2); }   // empty: both consumers
         fence_barrier_init();
     }
@@ -428,26 +463,42 @@ conv_wgrad_pp_kernel(const __grid_constant__ CUtensorMap tmDz, const __grid_cons
                     at_i[q] = tap / a.kw;
                     at_j[q] = tap - at_i[q] * a.kw;
                 }
+                if (kb_lo == kb_hi) continue;
+                // The unit's first K block is decoded once; the loop then steps (column block, row, image block) and
+                // the segment, so the segment's fields stay in registers off the path from a free stage to its loads.
+                int sel = 0;
+                for (int q = 1; q < a.nseg; ++q) if (kb_lo >= a.seg[q].kb_begin) sel = q;
+                WgradSeg sg = a.seg[sel];
+                int next = sel + 1 < a.nseg ? a.seg[sel + 1].kb_begin : a.kb_total;
+                int r = kb_lo - sg.kb_begin;
+                int wb = r % sg.w_blocks;
+                r /= sg.w_blocks;
+                int ho = r % a.Ho, n = r / a.Ho * sg.bn;
+                const CUtensorMap *tdz = &tm.dz[sel], *tx = &tm.x[sel];
                 for (int kb = kb_lo; kb < kb_hi; ++kb, ++it) {
+                    if (kb == next) {
+                        ++sel;
+                        sg = a.seg[sel];
+                        next = sel + 1 < a.nseg ? a.seg[sel + 1].kb_begin : a.kb_total;
+                        wb = 0; ho = 0; n = 0;
+                        tdz = &tm.dz[sel]; tx = &tm.x[sel];
+                    }
                     const int s = it % STAGES;
                     mbar_wait(empty + s, ((it / STAGES) & 1) ^ 1);
-                    int r = kb;
-                    const int wb = r % a.wboxes; r /= a.wboxes;
-                    const int ho = r % a.Ho;
-                    const int n = r / a.Ho;
+                    const int w = sg.w0 + wb * sg.bw;
                     unsigned char *a_dst = smem + s * L::STAGE_BYTES;
                     unsigned char *b_dst = a_dst + L::A_BYTES;
                     mbar_expect_tx(full + s, L::STAGE_BYTES);
-                    tma_load_4d(&tmDz, full + s, a_dst, m0, wb * RB, ho, n);
-                    tma_load_4d(&tmDz, full + s, a_dst + L::ATOM, m0 + 64, wb * RB, ho, n);
+                    tma_load_4d(tdz, full + s, a_dst, m0, w, ho, n);
+                    tma_load_4d(tdz, full + s, a_dst + L::ATOM, m0 + 64, w, ho, n);
 #pragma unroll
                     for (int q = 0; q < 4; ++q) {
                         if (n0 + 64 * q < a.K)
-                            tma_load_4d(&tmX, full + s, b_dst + q * L::ATOM, at_c[q], wb * RB + at_j[q] - a.pw,
-                                        ho + at_i[q] - a.ph, n);
+                            tma_load_4d(tx, full + s, b_dst + q * L::ATOM, at_c[q], w + at_j[q] - a.pw, ho + at_i[q] - a.ph, n);
                         else   // column atom beyond kh*kw*C: keep the transaction count with an all-out-of-bounds box
-                            tma_load_4d(&tmX, full + s, b_dst + q * L::ATOM, 0, -RB - 8, 0, n);
+                            tma_load_4d(tx, full + s, b_dst + q * L::ATOM, 0, -256, 0, n);
                     }
+                    if (++wb == sg.w_blocks) { wb = 0; if (++ho == a.Ho) { ho = 0; n += sg.bn; } }
                 }
             }
         }
@@ -524,12 +575,48 @@ int launch_m256(const CUtensorMap &tb, const CUtensorMap *tx, const CUtensorMap 
 }
 
 template <int RB>
-int launch_wgrad_pp(const CUtensorMap &tdz, const CUtensorMap &tx, float *dW, const PpWgradArgs &a, int grid,
-                    cudaStream_t st) {
+int launch_wgrad_pp(const WgradMaps &tm, float *dW, const PpWgradArgs &a, int grid, cudaStream_t st) {
     auto kern = conv_wgrad_pp_kernel<RB>;
     { int rc = ensure_dyn_smem((const void *)kern, PpWgradSmem<RB>::TOTAL, "conv_wgrad_pp smem attr"); if (rc) return rc; }
-    kern<<<grid, kPpThreads, PpWgradSmem<RB>::TOTAL, st>>>(tdz, tx, dW, a);
+    kern<<<grid, kPpThreads, PpWgradSmem<RB>::TOTAL, st>>>(tm, dW, a);
     return check_launch("conv_wgrad_pp_kernel");
+}
+
+// The weight gradient's schedule on at most `ctas` (>= 1) CTAs: segments, tiles, splits and grid.  *balanced: every CTA
+// gets the same number of units.
+int plan_wgrad(int N, int Ho, int Wo, int C, int Cout, int kh, int kw, int ph, int pw, int ctas, int min_kb, PpWgradArgs *pa,
+               int *grid_out, bool *balanced) {
+    PpWgradArgs &a = *pa;
+    a.C = C; a.Cout = Cout; a.K = kh * kw * C; a.kw = kw; a.ph = ph; a.pw = pw; a.Ho = Ho;
+    const int64_t kb_total = plan_wgrad_segments(N, Ho, Wo, wgrad_rb(Wo), a.seg, &a.nseg);
+    a.n_tiles = (int)ceil_div(a.K, 256);
+    const int64_t tiles = ceil_div(Cout, BM) * a.n_tiles;
+    if (kb_total * tiles > (1LL << 31) / 2) return MR_ERR_UNSUPPORTED;
+    a.kb_total = (int)kb_total;
+    a.tiles = (int)tiles;
+    if (ctas > kb_total * tiles) ctas = (int)(kb_total * tiles);
+    if (min_kb < 1) min_kb = 1;
+    /* The plan makes splits x tiles a whole multiple of the grid, and lets the grid go down to 90 % of `ctas` for it:
+     * (1) one unit per CTA, splits = ctas / tiles, when that fills 90 % of the CTAs;
+     * (2) otherwise the largest such grid g whose fewest splits, g / gcd(g, tiles), keep min_kb K blocks each;
+     * (3) otherwise (few K blocks, or few CTAs) ctas / tiles splits, as many as min_kb allows, and some CTAs get one unit
+     *     more than others. */
+    int64_t splits = std::min<int64_t>(kb_total, std::max<int64_t>(1, ctas / tiles));
+    int64_t grid = 0;
+    if (splits * tiles <= ctas && splits * tiles * 10 >= (int64_t)ctas * 9) grid = splits * tiles;
+    for (int g = ctas; grid == 0 && (int64_t)g * 10 >= (int64_t)ctas * 9; --g) {
+        const int64_t s = g / std::gcd<int64_t>(g, tiles);
+        if (kb_total >= s * min_kb) { splits = s; grid = g; }
+    }
+    *balanced = grid != 0;
+    if (grid == 0) {
+        splits = std::max<int64_t>(1, std::min<int64_t>(splits, kb_total / min_kb));
+        grid = std::min<int64_t>(ctas, splits * tiles);
+    }
+    a.kb_split = (int)ceil_div(kb_total, splits);
+    a.units = (int)(splits * tiles);
+    *grid_out = (int)grid;
+    return MR_OK;
 }
 
 }  // namespace
@@ -601,47 +688,48 @@ int mr_conv_wgrad_pp(const void *dz, const void *x, float *dWm, int N, int H, in
     if (N == 0) return MR_OK;
     if (!dz || !x || !dWm) return MR_ERR_NULL_POINTER;
     if (C % 64 || Cout % 8 || ((uintptr_t)x % 16) || ((uintptr_t)dz % 16) || ((uintptr_t)dWm % 16)) return MR_ERR_UNSUPPORTED;
-    const bool rb80 = Wo > 64 && Wo <= 80;
-    const int RB = rb80 ? 80 : 64;
-    PpWgradArgs a;
-    a.C = C; a.Cout = Cout; a.K = kh * kw * C; a.kw = kw; a.ph = ph; a.pw = pw; a.Ho = Ho;
-    a.wboxes = (int)ceil_div(Wo, RB);
-    a.n_tiles = (int)ceil_div(a.K, 256);
-    const int64_t kb_total = (int64_t)N * Ho * a.wboxes;
-    const int64_t tiles = ceil_div(Cout, BM) * a.n_tiles;
-    if (kb_total * tiles > (1LL << 31) / 2) return MR_ERR_UNSUPPORTED;
-    a.kb_total = (int)kb_total;
-    a.tiles = (int)tiles;
     const int sms = sm_count();
+    if (sms <= 0) { set_cuda_error(cudaErrorUnknown, "multiprocessor count"); return MR_ERR_CUDA; }
     if (ctas <= 0 || ctas > sms) ctas = sms;
-    if (ctas > kb_total * tiles) ctas = (int)(kb_total * tiles);
-    if (min_kb < 1) min_kb = 1;
-    /* The plan makes splits x tiles a whole multiple of the grid, and lets the grid go down to 90 % of `ctas` for it:
-     * (1) one unit per CTA, splits = ctas / tiles, when that fills 90 % of the CTAs;
-     * (2) otherwise the largest such grid g whose fewest splits, g / gcd(g, tiles), keep min_kb K blocks each;
-     * (3) otherwise (few K blocks, or few CTAs) ctas / tiles splits, as many as min_kb allows, and some CTAs get one unit
-     *     more than others. */
-    int64_t splits = std::min<int64_t>(kb_total, std::max<int64_t>(1, ctas / tiles));
-    int64_t grid = 0;
-    if (splits * tiles <= ctas && splits * tiles * 10 >= (int64_t)ctas * 9) grid = splits * tiles;
-    for (int g = ctas; grid == 0 && (int64_t)g * 10 >= (int64_t)ctas * 9; --g) {
-        const int64_t s = g / std::gcd<int64_t>(g, tiles);
-        if (kb_total >= s * min_kb) { splits = s; grid = g; }
-    }
-    if (grid == 0) {
-        splits = std::max<int64_t>(1, std::min<int64_t>(splits, kb_total / min_kb));
-        grid = std::min<int64_t>(ctas, splits * tiles);
-    }
-    a.kb_split = (int)ceil_div(kb_total, splits);
-    a.units = (int)(splits * tiles);
-    CUtensorMap tdz, tx;
-    int rc = make_map_nhwc(&tdz, dz, Cout, Wo, Ho, N, RB);
+    PpWgradArgs a;
+    int grid = 0;
+    bool balanced = false;
+    int rc = plan_wgrad(N, Ho, Wo, C, Cout, kh, kw, ph, pw, ctas, min_kb, &a, &grid, &balanced);
     if (rc) return rc;
-    rc = make_map_nhwc(&tx, x, C, W, H, N, RB);
-    if (rc) return rc;
+    WgradMaps tm;
+    for (int q = 0; q < kMaxWgradSegs; ++q) {
+        const WgradSeg &s = a.seg[q < a.nseg ? q : 0];
+        rc = make_map_nhwc(&tm.dz[q], dz, Cout, Wo, Ho, N, s.bw, 1, s.bn);
+        if (rc) return rc;
+        rc = make_map_nhwc(&tm.x[q], x, C, W, H, N, s.bw, 1, s.bn);
+        if (rc) return rc;
+    }
     cudaStream_t st = (cudaStream_t)stream;
-    return rb80 ? launch_wgrad_pp<80>(tdz, tx, dWm, a, (int)grid, st)
-                : launch_wgrad_pp<64>(tdz, tx, dWm, a, (int)grid, st);
+    return wgrad_rb(Wo) == 80 ? launch_wgrad_pp<80>(tm, dWm, a, grid, st) : launch_wgrad_pp<64>(tm, dWm, a, grid, st);
+}
+
+/* Host only: the schedule mr_conv_wgrad_pp runs on `ctas` (>= 1) CTAs, into plan[MR_WGRAD_PP_PLAN_INTS]:
+ * {RB, grid, kb_total, tiles, kb_split, units, balanced, nseg, then nseg x (w0, bw, bn, w_blocks, kb_begin)}. */
+int mr_conv_wgrad_pp_plan(int N, int H, int W, int C, int Cout, int kh, int kw, int ph, int pw, int ctas, int min_kb,
+                          int *plan) {
+    if (N <= 0 || H <= 0 || W <= 0 || C <= 0 || Cout <= 0 || kh <= 0 || kw <= 0 || ph < 0 || pw < 0 || ctas <= 0)
+        return MR_ERR_BAD_SHAPE;
+    const int Ho = H + 2 * ph - kh + 1, Wo = W + 2 * pw - kw + 1;
+    if (Ho <= 0 || Wo <= 0) return MR_ERR_BAD_SHAPE;
+    if (!plan) return MR_ERR_NULL_POINTER;
+    PpWgradArgs a;
+    int grid = 0;
+    bool balanced = false;
+    const int rc = plan_wgrad(N, Ho, Wo, C, Cout, kh, kw, ph, pw, ctas, min_kb, &a, &grid, &balanced);
+    if (rc) return rc;
+    int *p = plan;
+    *p++ = wgrad_rb(Wo); *p++ = grid; *p++ = a.kb_total; *p++ = a.tiles; *p++ = a.kb_split; *p++ = a.units;
+    *p++ = balanced; *p++ = a.nseg;
+    for (int q = 0; q < kMaxWgradSegs; ++q) {
+        const WgradSeg s = q < a.nseg ? a.seg[q] : WgradSeg{0, 0, 0, 0, 0};
+        *p++ = s.w0; *p++ = s.bw; *p++ = s.bn; *p++ = s.w_blocks; *p++ = s.kb_begin;
+    }
+    return MR_OK;
 }
 
 }  // extern "C"

@@ -1,5 +1,7 @@
 """Thin torch-tensor wrappers over the C-ABI building blocks (include/megreader_b200.h, csrc/nn_kernels.cu,
 csrc/gemm.cu).  No arithmetic happens in Python; these only allocate outputs and pass pointers."""
+import ctypes
+import functools
 import os
 
 import torch
@@ -322,15 +324,38 @@ def conv_wgrad_pp(dz, x, kh, kw, ph, pw, out=None, ctas=None):
     dWm = out if out is not None else torch.zeros((Cout, K), dtype=torch.float32, device=x.device)
     if ctas is None:
         # One CTA per SM, as long as each CTA still owns _WGRAD_MIN_KB K blocks to amortise the atomic flush of a tile.
-        rb = 80 if 64 < Wo <= 80 else 64
-        work = N * Ho * -(-Wo // rb) * -(-Cout // 128) * -(-K // 256)
-        ctas = min(torch.cuda.get_device_properties(x.device).multi_processor_count, max(1, work // _WGRAD_MIN_KB))
+        ctas = 0
+        if N > 0:
+            sms = torch.cuda.get_device_properties(x.device).multi_processor_count
+            plan = conv_wgrad_pp_plan(N, H, W, C, Cout, kh, kw, ph, pw, sms)
+            if plan is None:
+                return None
+            ctas = min(sms, max(1, plan["kb_total"] * plan["tiles"] // _WGRAD_MIN_KB))
     rc = _lib.lib().mr_conv_wgrad_pp(_p(dz), _p(x), _p(dWm), N, H, W, C, Cout, kh, kw, ph, pw, int(ctas), _WGRAD_MIN_KB,
                                      _st())
     if rc == _lib.MR_ERR_UNSUPPORTED:
         return None
     _chk(rc, "conv_wgrad_pp")
     return dWm
+
+
+@functools.lru_cache(maxsize=256)
+def conv_wgrad_pp_plan(N, H, W, C, Cout, kh, kw, ph, pw, ctas, min_kb=None):
+    """The schedule conv_wgrad_pp runs on `ctas` CTAs (host only, no device): a dict with RB (output pixels per K block),
+    grid, kb_total (K blocks per tile), tiles (128 x 256 tiles), kb_split, units, balanced (every CTA gets the same number
+    of units) and segs, a list of (w0, bw, bn, w_blocks, kb_begin): the K blocks of a segment are boxes of bw columns x 1
+    row x bn images.  None when the entry refuses the geometry."""
+    plan = (ctypes.c_int * 33)()                      # MR_WGRAD_PP_PLAN_INTS
+    rc = _lib.lib().mr_conv_wgrad_pp_plan(N, H, W, C, Cout, kh, kw, ph, pw, int(ctas),
+                                          _WGRAD_MIN_KB if min_kb is None else int(min_kb), plan)
+    if rc == _lib.MR_ERR_UNSUPPORTED:
+        return None
+    _chk(rc, "conv_wgrad_pp_plan")
+    v = list(plan)
+    out = dict(zip(("RB", "grid", "kb_total", "tiles", "kb_split", "units", "balanced", "nseg"), v[:8]))
+    out["balanced"] = bool(out["balanced"])
+    out["segs"] = [tuple(v[8 + 5 * q: 13 + 5 * q]) for q in range(out.pop("nseg"))]
+    return out
 
 
 def conv_wgrad_tc(dz, x, kh, kw, ph, pw, splits=0, out=None):
