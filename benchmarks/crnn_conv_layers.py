@@ -15,7 +15,8 @@ bf16 NHWC activations).
 (c) the persistent kernels against each other, call by call, the arms alternating round after round: forward and input
     gradient on the 128-pixel ping-pong kernel (tile_m=128) and as mr_conv_fprop_pp selects (tile_m=0: the 256-pixel
     kernel from 36 K blocks on), L6's input gradient also as the engine's row split (two 1 x 2 convolutions), and the
-    weight gradient with the planner's schedule (its old arm is this script's (a) run from the parent build).  Beside
+    weight gradient with the planner's schedule on 128 x 256 tiles (its old arm is this script's (a) run from the parent
+    build) and, at L1 and L2, as the engine runs it (crnn_engine._conv_wgrad: 128 x 192 tiles).  Beside
     TFLOP/s it prints the L2-to-SM rate implied by the kernel's operand bytes per FLOP, and for the weight gradient the
     share of the issued MMA work that multiplies real pixels and columns rather than zero fill.
         python benchmarks/crnn_conv_layers.py --changed --out DIR [--batch 512] [--rounds 3]
@@ -114,7 +115,7 @@ def run_layers(args):
 # operand bytes loaded from L2 per FLOP: a 64-deep K block of a 128 x 128 tile (ping-pong), of two 128-pixel tiles sharing
 # one 128-wide weight box (256-pixel kernel), of a 128 x 256 weight-gradient tile (RB rows: the same ratio)
 B_PER_FLOP = {"pp128": 32768 / (2 * 128 * 128 * 64), "m256": 49152 / (2 * 256 * 128 * 64),
-              "wgrad": (128 + 256) * 128 / (2 * 128 * 256 * 64)}
+              "wgrad": (128 + 256) * 128 / (2 * 128 * 256 * 64), "wgrad_n192": (128 + 192) * 128 / (2 * 128 * 192 * 64)}
 
 
 def changed_calls(n, dev):
@@ -140,18 +141,23 @@ def changed_calls(n, dev):
                 arms["rows"] = (lambda a=a, w=w, k=k, p=p, H=H: crnn_engine._conv_dgrad(a, w, k, k, p, p, H),
                                 B_PER_FLOP["pp128"])
             out.append((name, kind, flop, arms))
-        out.append((name, "wgrad", flop, {"selected": (lambda dz=dz, x=x, k=k, p=p, dW=dW: ops.conv_wgrad_pp(
-            dz, x, k, k, p, p, out=dW.zero_()), B_PER_FLOP["wgrad"])}))
+        arms = {"selected": (lambda dz=dz, x=x, k=k, p=p, dW=dW: ops.conv_wgrad_pp(dz, x, k, k, p, p, out=dW.zero_()),
+                             B_PER_FLOP["wgrad"])}
+        if k * k * C % 256 and k * k * C % 192 == 0:  # the engine runs these on 128 x 192 tiles
+            arms["engine"] = (lambda dz=dz, x=x, k=k, p=p, dW=dW: crnn_engine._conv_wgrad(dz, x, k, k, p, p, out=dW.zero_()),
+                              B_PER_FLOP["wgrad_n192"])
+        out.append((name, "wgrad", flop, arms))
     return out
 
 
-def wgrad_useful_mma(name, n, sms):
+def wgrad_useful_mma(name, n, sms, n192=False):
     """Share of the weight gradient's issued MMA work that multiplies real operands: the useful products over the K blocks
-    (RB pixels each, zero fill included) x 128 x 256 tiles of mr_conv_wgrad_pp's plan."""
+    (RB pixels each, zero fill included) x 128 x 256 tiles of mr_conv_wgrad_pp's plan (n192: x 128 x 192 tiles of
+    mr_conv_wgrad_n192's)."""
     _, H, W, C, Cout, k, p = next(lay for lay in LAYERS if lay[0] == name)
     Ho, Wo = H + 2 * p - k + 1, W + 2 * p - k + 1
-    plan = ops.conv_wgrad_pp_plan(n, H, W, C, Cout, k, k, p, p, sms)
-    return n * Ho * Wo * Cout * k * k * C / (plan["kb_total"] * plan["RB"] * plan["tiles"] * 128 * 256)
+    plan = (ops.conv_wgrad_n192_plan if n192 else ops.conv_wgrad_pp_plan)(n, H, W, C, Cout, k, k, p, p, sms)
+    return n * Ho * Wo * Cout * k * k * C / (plan["kb_total"] * plan["RB"] * plan["tiles"] * 128 * (192 if n192 else 256))
 
 
 def run_changed(args):
@@ -178,13 +184,16 @@ def run_changed(args):
                 row[arm]["same_bits_as_pp128"] = bool(torch.equal(r.view_as(ref), ref))
         if kind == "wgrad":
             row["useful_mma"] = wgrad_useful_mma(name, args.batch, sms)
+            if "engine" in arms:
+                row["engine"]["useful_mma"] = wgrad_useful_mma(name, args.batch, sms, n192=True)
         rows.append(row)
         print("%-3s %-6s %s" % (name, kind, "  ".join(
             "%s %7.1f us (%s) %6.1f TFLOP/s L2 %4.1f TB/s%s" % (
                 arm, v["us"], "/".join("%.0f" % u for u in v["us_all"]), v["tflops"], v["l2_tb_s"],
                 "" if v.get("same_bits_as_pp128", True) else " DIFFERENT")
             for arm, v in row.items() if isinstance(v, dict)) +
-            ("  useful MMA %.1f %% of issued" % (100 * row["useful_mma"]) if kind == "wgrad" else "")), flush=True)
+            ("  useful MMA %.1f %% of issued" % (100 * row["useful_mma"]) if kind == "wgrad" else "") +
+            (" (engine %.1f %%)" % (100 * row["engine"]["useful_mma"]) if "engine" in row else "")), flush=True)
     return {"batch": args.batch, "iters_per_graph": args.iters, "rounds": args.rounds, "calls": rows}
 
 

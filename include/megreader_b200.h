@@ -488,6 +488,11 @@ int mr_conv_wgrad_tcgen05(const void *dz, const void *x, float *dWm, int N, int 
  * output that tiles with at most four TMA box segments (the caller then uses mr_conv_fprop_tcgen05). */
 int mr_conv_fprop_pp(const void *x, const void *Wm, void *y, int N, int H, int W, int C, int Cout, int kh, int kw, int ph,
                      int pw, int ldw, int y_nstride, int tile_m, void *stream);
+/* Host only: 1 when mr_conv_fprop_pp runs this geometry (tile_m = 0 or 128) in the ping-pong kernel's halo mode, which
+ * loads one (128 + kw - 1)-pixel activation halo per tap row and channel block and runs the row's kw taps from it (same
+ * bits, a third of the activation bytes at kw = 3): Wo a multiple of 128 (at most 512), 2 <= kw <= 8, C <= 256.  0 when it
+ * does not; MR_ERR_BAD_SHAPE for an invalid geometry. */
+int mr_conv_fprop_pp_halo(int H, int W, int C, int Cout, int kh, int kw, int ph, int pw);
 /* Weight gradient of the same convolutions on a persistent wgmma kernel with 128 x 256 tiles (csrc/conv_pingpong.cu):
  * dWm[Cout, kh*kw*C] fp32 += dz[N,Ho,Wo,Cout]^T (*) x[N,H,W,C], ACCUMULATED atomically (zero it first).  The K blocks of
  * all tiles are cut into splits, and the (split, tile) units are handed out to at most `ctas` CTAs (<= 0: one per SM),
@@ -505,6 +510,14 @@ int mr_conv_wgrad_pp(const void *dz, const void *x, float *dWm, int N, int H, in
 #define MR_WGRAD_PP_PLAN_INTS 33
 int mr_conv_wgrad_pp_plan(int N, int H, int W, int C, int Cout, int kh, int kw, int ph, int pw, int ctas, int min_kb,
                           int *plan);
+/* mr_conv_wgrad_pp with 128 x 192 tiles: both consumer warpgroups multiply one 192-column x stage, each by its own 64 rows
+ * of dz.  Where kh*kw*C is a multiple of 192 but not of 256 (576 and 1152 at the CRNN's first two 3x3 layers) no column
+ * of an issued tile lies beyond kh*kw*C.  Same arguments, accumulation and refusals as mr_conv_wgrad_pp. */
+int mr_conv_wgrad_n192(const void *dz, const void *x, float *dWm, int N, int H, int W, int C, int Cout, int kh, int kw, int ph,
+                       int pw, int ctas, int min_kb, void *stream);
+/* Host only: the schedule mr_conv_wgrad_n192 runs, in mr_conv_wgrad_pp_plan's layout; `tiles` counts 128 x 192 tiles. */
+int mr_conv_wgrad_n192_plan(int N, int H, int W, int C, int Cout, int kh, int kw, int ph, int pw, int ctas, int min_kb,
+                            int *plan);
 
 /* Fused LSTM time steps on wgmma (recurrent GEMM + cell in one launch, both directions): gate columns are
  * UNIT-MAJOR (column 4*j + g = gate g in {i,f,g,o} of hidden unit j), H % 64 == 0, bf16.  Every per-direction argument

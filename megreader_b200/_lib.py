@@ -57,8 +57,11 @@ _SIGS = {
     "mr_conv2d_fprop_tcgen05": [c_p] * 3 + [c_int] * 14 + [c_p, c_int, c_p],
     "mr_conv2d_wgrad_tcgen05": [c_p] * 3 + [c_int] * 14 + [c_p],
     "mr_conv_fprop_pp": [c_p] * 3 + [c_int] * 12 + [c_p],
+    "mr_conv_fprop_pp_halo": [c_int] * 8,
     "mr_conv_wgrad_pp": [c_p] * 3 + [c_int] * 11 + [c_p],
     "mr_conv_wgrad_pp_plan": [c_int] * 11 + [c_p],
+    "mr_conv_wgrad_n192": [c_p] * 3 + [c_int] * 11 + [c_p],
+    "mr_conv_wgrad_n192_plan": [c_int] * 11 + [c_p],
     "mr_lstm_step_fwd_tcgen05": [c_p] * 7 + [c_i64, c_p, c_int, c_int, c_int, c_p],
     "mr_lstm_step_bwd_tcgen05": [c_p] * 6 + [c_i64, c_p, c_p, c_int, c_int, c_int, c_p],
     "mr_lstm_seq_fwd_tcgen05": [c_p] * 6 + [c_int] * 3 + [c_p],

@@ -135,9 +135,12 @@ def _conv_dgrad(dz, Wd, kh, kw, ph, pw, H):
 
 
 def _conv_wgrad(dz, x, kh, kw, ph, pw, out=None):
-    """Weight gradient [Cout, kh*kw*C] fp32 (accumulated into a zeroed `out` if given) on the persistent 128 x 256 kernel;
-    the one-tile-per-CTA kernel only for geometries the former refuses."""
-    r = ops.conv_wgrad_pp(dz, x, kh, kw, ph, pw, out=out)
+    """Weight gradient [Cout, kh*kw*C] fp32 (accumulated into a zeroed `out` if given) on a persistent kernel: 128 x 192
+    tiles where K = kh*kw*C is a multiple of 192 but not of 256 (L1, L2: K = 576, 1152, which 256-column tiles issue as 768
+    and 1280 columns), 128 x 256 tiles otherwise; the one-tile-per-CTA kernel only for geometries they refuse."""
+    K = kh * kw * x.size(3)
+    persistent = ops.conv_wgrad_n192 if K % 256 and K % 192 == 0 else ops.conv_wgrad_pp
+    r = persistent(dz, x, kh, kw, ph, pw, out=out)
     return r if r is not None else ops.conv_wgrad_tc(dz, x, kh, kw, ph, pw, out=out)
 
 

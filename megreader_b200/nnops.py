@@ -314,10 +314,29 @@ def conv_fprop_pp(x, Wm, kh, kw, ph, pw, tile_m=0, out=None):
     return y, Ho, Wo
 
 
+def conv_fprop_pp_halo(H, W, C, Cout, kh, kw, ph, pw):
+    """Host only: True when conv_fprop_pp (tile_m 0 or 128) runs this geometry in the ping-pong kernel's halo mode, which
+    loads one activation halo per tap row and channel block and runs the row's kw taps from it (same bits)."""
+    rc = _lib.lib().mr_conv_fprop_pp_halo(H, W, C, Cout, kh, kw, ph, pw)
+    if rc not in (0, 1):
+        _chk(rc, "conv_fprop_pp_halo")
+    return rc == 1
+
+
 def conv_wgrad_pp(dz, x, kh, kw, ph, pw, out=None, ctas=None):
     """dWm [Cout, kh*kw*C] fp32 from dz [N,Ho,Wo,Cout] and x [N,H,W,C] (NHWC bf16) on the persistent 128 x 256 wgmma kernel
     (csrc/conv_pingpong.cu); `out`: a ZEROED [Cout, K] fp32 buffer to accumulate into.  None when the entry refuses the
     geometry (MR_ERR_UNSUPPORTED): the caller then uses conv_wgrad_tc.  `ctas` caps the grid (default below)."""
+    return _conv_wgrad_persistent("conv_wgrad_pp", conv_wgrad_pp_plan, dz, x, kh, kw, ph, pw, out, ctas)
+
+
+def conv_wgrad_n192(dz, x, kh, kw, ph, pw, out=None, ctas=None):
+    """conv_wgrad_pp on the kernel with 128 x 192 tiles (csrc/conv_pingpong.cu, conv_wgrad_n192_kernel): no idle column
+    atoms where kh*kw*C is a multiple of 192 but not of 256 (the CRNN's L1 and L2)."""
+    return _conv_wgrad_persistent("conv_wgrad_n192", conv_wgrad_n192_plan, dz, x, kh, kw, ph, pw, out, ctas)
+
+
+def _conv_wgrad_persistent(entry, plan_fn, dz, x, kh, kw, ph, pw, out, ctas):
     N, H, W, C = x.shape
     _, Ho, Wo, Cout = dz.shape
     K = kh * kw * C
@@ -327,15 +346,15 @@ def conv_wgrad_pp(dz, x, kh, kw, ph, pw, out=None, ctas=None):
         ctas = 0
         if N > 0:
             sms = torch.cuda.get_device_properties(x.device).multi_processor_count
-            plan = conv_wgrad_pp_plan(N, H, W, C, Cout, kh, kw, ph, pw, sms)
+            plan = plan_fn(N, H, W, C, Cout, kh, kw, ph, pw, sms)
             if plan is None:
                 return None
             ctas = min(sms, max(1, plan["kb_total"] * plan["tiles"] // _WGRAD_MIN_KB))
-    rc = _lib.lib().mr_conv_wgrad_pp(_p(dz), _p(x), _p(dWm), N, H, W, C, Cout, kh, kw, ph, pw, int(ctas), _WGRAD_MIN_KB,
-                                     _st())
+    rc = getattr(_lib.lib(), "mr_" + entry)(_p(dz), _p(x), _p(dWm), N, H, W, C, Cout, kh, kw, ph, pw, int(ctas),
+                                            _WGRAD_MIN_KB, _st())
     if rc == _lib.MR_ERR_UNSUPPORTED:
         return None
-    _chk(rc, "conv_wgrad_pp")
+    _chk(rc, entry)
     return dWm
 
 
@@ -345,12 +364,22 @@ def conv_wgrad_pp_plan(N, H, W, C, Cout, kh, kw, ph, pw, ctas, min_kb=None):
     grid, kb_total (K blocks per tile), tiles (128 x 256 tiles), kb_split, units, balanced (every CTA gets the same number
     of units) and segs, a list of (w0, bw, bn, w_blocks, kb_begin): the K blocks of a segment are boxes of bw columns x 1
     row x bn images.  None when the entry refuses the geometry."""
+    return _wgrad_plan("conv_wgrad_pp_plan", N, H, W, C, Cout, kh, kw, ph, pw, ctas, min_kb)
+
+
+@functools.lru_cache(maxsize=256)
+def conv_wgrad_n192_plan(N, H, W, C, Cout, kh, kw, ph, pw, ctas, min_kb=None):
+    """The schedule conv_wgrad_n192 runs, as conv_wgrad_pp_plan gives it; `tiles` counts 128 x 192 tiles."""
+    return _wgrad_plan("conv_wgrad_n192_plan", N, H, W, C, Cout, kh, kw, ph, pw, ctas, min_kb)
+
+
+def _wgrad_plan(entry, N, H, W, C, Cout, kh, kw, ph, pw, ctas, min_kb):
     plan = (ctypes.c_int * 33)()                      # MR_WGRAD_PP_PLAN_INTS
-    rc = _lib.lib().mr_conv_wgrad_pp_plan(N, H, W, C, Cout, kh, kw, ph, pw, int(ctas),
-                                          _WGRAD_MIN_KB if min_kb is None else int(min_kb), plan)
+    rc = getattr(_lib.lib(), "mr_" + entry)(N, H, W, C, Cout, kh, kw, ph, pw, int(ctas),
+                                            _WGRAD_MIN_KB if min_kb is None else int(min_kb), plan)
     if rc == _lib.MR_ERR_UNSUPPORTED:
         return None
-    _chk(rc, "conv_wgrad_pp_plan")
+    _chk(rc, entry)
     v = list(plan)
     out = dict(zip(("RB", "grid", "kb_total", "tiles", "kb_split", "units", "balanced", "nseg"), v[:8]))
     out["balanced"] = bool(out["balanced"])
