@@ -60,6 +60,11 @@ struct StemGeo {
 };
 
 __device__ __forceinline__ float bf16r(float v) { return __bfloat162float(__float2bfloat16_rn(v)); }
+__device__ __forceinline__ float fmax_nan(float a, float b) {      // max that returns NaN if either operand is NaN
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
 
 // ------------------------------------------------------------------------------------------------ forward
 // staged input: [SR][SC][4] bf16, channel 3 zero; staged (r, s) is input pixel (h0 - 1 + r, w0 - 1 + s), zero outside
@@ -155,9 +160,10 @@ crnn_stem_fwd_kernel(StemGeo g, const float *__restrict__ x, const float *__rest
                     best[e] = -INFINITY;
                     bi[e] = 0;
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        const float a = bf16r(fmaxf(bf16r(win[k]) + b, 0.f));
-                        if (a > best[e]) { best[e] = a; bi[e] = (unsigned char)k; }
+                    for (int k = 0; k < 4; ++k) {       // ReLU and max keep a NaN, as ATen's relu and max_pool2d do
+                        const float a = bf16r(fmax_nan(bf16r(win[k]) + b, 0.f));
+                        if (!(a <= best[e])) bi[e] = (unsigned char)k;
+                        best[e] = fmax_nan(best[e], a);
                     }
                     if (!(best[e] > 0.f)) bi[e] = kNotPositive;
                 }

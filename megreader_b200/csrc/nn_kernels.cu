@@ -261,8 +261,22 @@ __global__ void col2im_vec_kernel(ConvGeo g, const T *__restrict__ dcol, T *__re
 // ---------------------------------------------------------------- bias + ReLU (+ max-pool) on a GEMM output
 struct PoolGeo { int N, H, W, C, kh, kw, sh, sw, ph, pw, Ho, Wo; };
 
-// y[n,ho,wo,c] = max over window of relu(x + bias) ; idx = first arg-max in (i,j) scan order (ATen's strict '>').
-// Padded positions never win (ATen pads with -inf).  x is the raw GEMM output [N*H*W, C].
+// ReLU and max-pool that keep NaN like ATen's relu and max_pool2d (fmaxf would turn a NaN into 0 and a strict '>' never
+// takes one), so a diverged step stays visible.  max.NaN is one instruction, as fmaxf is.
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+    float r;
+    asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+    return r;
+}
+// One window position of the pool: the arg-max byte moves on a strictly larger value (ATen's '>': the first maximum
+// wins) or a NaN; the value keeps a NaN once taken.  The byte of a NaN window may differ from ATen's: it routes nothing.
+__device__ __forceinline__ void pool_step(float a, int k, float &best, int &bi) {
+    if (!(a <= best)) bi = k;
+    best = fmax_nan(best, a);
+}
+
+// y[n,ho,wo,c] = max over window of relu(x + bias) ; idx = first arg-max in (i,j) scan order.  Padded positions never
+// win (ATen pads with -inf).  x is the raw GEMM output [N*H*W, C].
 template <typename T>
 __global__ void bias_relu_pool_fwd_kernel(PoolGeo g, const T *__restrict__ x, const float *__restrict__ bias,
                                           T *__restrict__ y, unsigned char *__restrict__ idx) {
@@ -299,8 +313,7 @@ __global__ void bias_relu_pool_fwd_kernel(PoolGeo g, const T *__restrict__ x, co
 #pragma unroll
                 for (int e = 0; e < VN; ++e) {
                     // round through T so that the compared values are what an unfused bias+ReLU would have stored
-                    const float a = to_f<T>(from_f<T>(fmaxf(f[e] + bb[e], 0.f)));
-                    if (a > best[e]) { best[e] = a; bi[e] = i * g.kw + j; }
+                    pool_step(to_f<T>(from_f<T>(fmax_nan(f[e] + bb[e], 0.f))), i * g.kw + j, best[e], bi[e]);
                 }
             }
         }
@@ -313,7 +326,7 @@ __global__ void bias_relu_pool_fwd_kernel(PoolGeo g, const T *__restrict__ x, co
 }
 
 // dz[n,h,w,c] (gradient w.r.t. the raw GEMM output) = sum over windows that contain (h,w) whose arg-max is (h,w)
-// and whose pooled value is > 0 (ReLU') of dy[window].
+// and whose pooled value is > 0 (ReLU') of dy[window].  A NaN pooled value passes nothing, as ATen's threshold_backward.
 template <typename T>
 __global__ void __launch_bounds__(256)
 bias_relu_pool_bwd_kernel(PoolGeo g, const T *__restrict__ dy, const T *__restrict__ y,
@@ -463,8 +476,7 @@ pool_fwd_rows_kernel(PoolGeo g, const T *__restrict__ x, const float *__restrict
                 unpack<T>(v[k], f);
 #pragma unroll
                 for (int e = 0; e < VN; ++e) {
-                    const float a = to_f<T>(from_f<T>(fmaxf(f[e] + bb[e], 0.f)));
-                    if (a > best[e]) { best[e] = a; bi[e] = k; }
+                    pool_step(to_f<T>(from_f<T>(fmax_nan(f[e] + bb[e], 0.f))), k, best[e], bi[e]);
                 }
             }
             const int64_t t = ((int64_t)row * g.Wo + wo) * cv + cvec;
@@ -709,10 +721,17 @@ __global__ void bias_act_scalar_kernel(const T *__restrict__ x, const float *__r
 }
 
 // ---------------------------------------------------------------- per-channel reductions over rows
-// sums[0][c] += sum_r f(x[r,c] (+bias[c]));  sums[1][c] += sum_r g(...)   MODE 0: (x+b, (x+b)^2)   [BN statistics]
+// sums[0][c] += sum_r f(x[r,c] (+bias[c]));  sums[1][c] += sum_r g(...)   MODE 0: (s, s^2)           [BN statistics]
 //                                                                          MODE 1: (dy, dy*xhat)      [BN backward]
 //                                                                          MODE 2: (dy, -)            [bias gradient]
-// xhat = (x + bias - mean) * invstd.  One CTA = 32 channel-vectors x 8 row lanes; double atomics at the end.
+// xhat = (x + bias - mean) * invstd.  MODE 0 sums the shifted value s = x + b - K with K = x[0,c] + b[c] (bn_shift):
+// plain sums of x + b and (x + b)^2 in fp32 lose the variance to cancellation once |mean| >> std, shifted ones do not.
+// One CTA = 32 channel-vectors x 8 row lanes; double atomics at the end.
+template <typename T>
+__device__ __forceinline__ float bn_shift(const T *__restrict__ x, const float *__restrict__ bias, int c) {
+    return to_f<T>(x[c]) + (bias ? bias[c] : 0.f);
+}
+
 template <typename T, int MODE>
 __global__ void __launch_bounds__(256)
 col_reduce_kernel(const T *__restrict__ a, const T *__restrict__ b, const float *__restrict__ bias,
@@ -732,7 +751,7 @@ col_reduce_kernel(const T *__restrict__ a, const T *__restrict__ b, const float 
 #pragma unroll
         for (int e = 0; e < VN; ++e) {
             bb[e] = bias ? bias[v * VN + e] : 0.f;
-            mm[e] = (MODE == 1) ? mean[v * VN + e] : 0.f;
+            mm[e] = (MODE == 1) ? mean[v * VN + e] : (MODE == 0) ? bn_shift(a, bias, v * VN + e) : 0.f;
             is[e] = (MODE == 1) ? invstd[v * VN + e] : 0.f;
         }
         constexpr int U = 4;             // rows in flight per thread
@@ -752,7 +771,7 @@ col_reduce_kernel(const T *__restrict__ a, const T *__restrict__ b, const float 
                 unpack<T>(ra[k], fa);
                 if (MODE == 0) {
 #pragma unroll
-                    for (int e = 0; e < VN; ++e) { const float x = fa[e] + bb[e]; s0[e] += x; s1[e] += x * x; }
+                    for (int e = 0; e < VN; ++e) { const float x = (fa[e] + bb[e]) - mm[e]; s0[e] += x; s1[e] += x * x; }
                 } else if (MODE == 1) {
                     float fb[VN];
                     unpack<T>(rb[k], fb);
@@ -786,15 +805,19 @@ col_reduce_kernel(const T *__restrict__ a, const T *__restrict__ b, const float 
     }
 }
 
-// BatchNorm finalize (one thread per channel): mean / invstd from the sums, running-stat update (momentum, unbiased
-// variance for running_var like ATen), num_batches_tracked is bumped by the host.
-__global__ void bn_finalize_kernel(const double *__restrict__ sums, int64_t rows, int C, float eps, float momentum,
-                                   float *__restrict__ mean, float *__restrict__ invstd,
-                                   float *__restrict__ running_mean, float *__restrict__ running_var) {
+// BatchNorm finalize (one thread per channel): mean / invstd from the shifted sums of col_reduce_kernel<T, 0> (mean =
+// K + S1/n, var = S2/n - (S1/n)^2 with the same shift K), running-stat update (momentum, unbiased variance for
+// running_var like ATen), num_batches_tracked is bumped by the host.
+template <typename T>
+__global__ void bn_finalize_kernel(const double *__restrict__ sums, const T *__restrict__ x, const float *__restrict__ bias,
+                                   int64_t rows, int C, float eps, float momentum, float *__restrict__ mean,
+                                   float *__restrict__ invstd, float *__restrict__ running_mean,
+                                   float *__restrict__ running_var) {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
-    const double m = sums[c] / (double)rows;
-    double var = sums[C + c] / (double)rows - m * m;
+    const double d = sums[c] / (double)rows;
+    const double m = (double)bn_shift(x, bias, c) + d;
+    double var = sums[C + c] / (double)rows - d * d;
     if (var < 0) var = 0;
     mean[c] = (float)m;
     invstd[c] = (float)(1.0 / sqrt(var + (double)eps));
@@ -1446,7 +1469,8 @@ int mr_bn_train_fwd(const void *x, const float *bias, const float *gamma, const 
     cudaStream_t st = (cudaStream_t)stream;
     int rc = launch_reduce(0, dtype, x, nullptr, bias, nullptr, nullptr, rows, C, sums, st);
     if (rc) return rc;
-    bn_finalize_kernel<<<(int)ceil_div(C, 128), 128, 0, st>>>(sums, rows, C, eps, momentum, mean, invstd, running_mean, running_var);
+    DISPATCH(dtype, (bn_finalize_kernel<T><<<(int)ceil_div(C, 128), 128, 0, st>>>(sums, (const T *)x, bias, rows, C, eps, momentum,
+                                                                              mean, invstd, running_mean, running_var)));
     rc = check_launch("bn_finalize_kernel");
     if (rc) return rc;
     const int vn = dtype == 0 ? 4 : 8;

@@ -118,6 +118,33 @@ def test_backward_vs_float64_and_repeatable(cuda, shape):
 
 
 @pytest.mark.gpu
+def test_nan_weight_propagates_like_aten(cuda):
+    """One NaN weight makes its output channel NaN before the ReLU.  ATen's relu and max_pool2d keep the NaN, so the pooled
+    channel is NaN (not 0) and routes no gradient (threshold_backward); every other channel is unchanged."""
+    from megreader_b200 import nnops as ops
+    n, h, w = 3, 32, 48
+    conv = _conv(11, cuda)
+    co = 17
+    with torch.no_grad():
+        conv.weight[co, 1, 2, 0] = float("nan")
+    x, dy = _inputs(12, n, h, w, cuda)
+    y, idx = ops.crnn_stem_fwd(x, conv, POOL, True)
+    assert bool(torch.isnan(y[..., co]).all()), "a NaN pre-activation must survive ReLU + max-pool"
+    assert bool((idx[..., co] == 4).all())
+    want = F.max_pool2d(F.relu(F.conv2d(x, conv.weight, conv.bias, padding=1)), 2, 2)
+    assert bool(torch.isnan(want[:, co]).all())
+    keep = torch.arange(64, device=cuda) != co
+    y_ref, arg_ref, pre64, zmax = _reference_fwd(x, conv)
+    _check_fwd(y[..., keep], idx[..., keep], y_ref[..., keep], arg_ref[..., keep], pre64[..., keep, :],
+               zmax[..., keep])
+    assert not torch.isnan(y[..., keep]).any()
+    dw, db = ops.crnn_stem_bwd(x, dy, idx, conv, POOL)
+    dw_ref, db_ref = _reference_bwd(x, dy, idx)
+    assert bool((dw[co] == 0).all()) and float(db[co]) == 0.0
+    assert _rel(dw[keep], dw_ref[keep]) <= 1e-5 and _rel(db[keep], db_ref[keep]) <= 1e-5
+
+
+@pytest.mark.gpu
 def test_cuda_graph_replay_matches_eager(cuda):
     from megreader_b200 import nnops as ops
     conv = _conv(5, cuda)

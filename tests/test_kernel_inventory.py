@@ -1,5 +1,7 @@
 """CPU: the tensor-core kernel instantiations compiled into the library are exactly wgmma_variants.ALL_VARIANTS, and each
-of them is the expected kernel of at least one GPU test case -- a new instantiation without a test fails here."""
+of them is the expected kernel of at least one GPU test case -- a new instantiation without a test fails here.  The same
+for the CTC kernels (ctc_variants) and the streaming kernels of csrc/nn_kernels.cu (nn_variants)."""
+import os
 import re
 import shutil
 import subprocess
@@ -7,7 +9,9 @@ import subprocess
 import pytest
 
 from tests import ctc_variants as cv
+from tests import nn_variants as nv
 from tests import test_conv_tcgen05_gpu, test_ctc_variants_gpu, test_dcn_gpu, test_gemm_tcgen05_gpu, test_lstm_step_gpu
+from tests import test_decode_gpu, test_nn_kernels_gpu, test_nn_streaming_gpu
 from tests import wgmma_variants as wv
 
 
@@ -119,3 +123,77 @@ def test_dispatch_restatement():
                         "(anonymous namespace)::GemmArgs)") == "gemm_tcgen05_kernel<128,6,0,1>"
     assert wv.normalise("void <unnamed>::conv_wgrad_tcgen05_kernel<(int)64, (int)80, (int)6>(CUtensorMap_st)") \
         == "conv_wgrad_tcgen05_kernel<64,80,6>"
+
+
+@pytest.mark.skipif(shutil.which("cuobjdump") is None or shutil.which("cu++filt") is None,
+                    reason="needs cuobjdump and cu++filt from the CUDA toolkit")
+def test_compiled_nn_kernels_are_the_known_kernels(so_path):
+    """csrc/nn_kernels.cu: every compiled kernel is restated by nn_variants or tested through its own entry elsewhere"""
+    from megreader_b200 import build
+    found = {nv.nn_normalise(n) for n in compiled_kernels(os.path.join(build.OBJ, "nn_kernels.o"))}
+    known = nv.REACHABLE | set(nv.COVERED_ELSEWHERE)
+    assert len(nv.REACHABLE) == 56 and len(nv.COVERED_ELSEWHERE) == 7
+    assert found == known, "unknown: %s; not compiled: %s" % (sorted(found - known), sorted(known - found))
+
+
+def test_every_nn_kernel_has_a_gpu_case():
+    covered = test_nn_streaming_gpu.KERNELS
+    assert covered <= nv.REACHABLE, sorted(covered - nv.REACHABLE)
+    assert covered == nv.REACHABLE, "no GPU case expects %s" % sorted(nv.REACHABLE - covered)
+    for kernel, test in nv.COVERED_ELSEWHERE.items():
+        module, name = test.split("::")
+        mod = {"tests/test_decode_gpu.py": test_decode_gpu, "tests/test_nn_kernels_gpu.py": test_nn_kernels_gpu}[module]
+        assert callable(getattr(mod, name, None)), "%s: %s is gone" % (kernel, test)
+
+
+def test_nn_dispatch_restatement():
+    """spot checks of tests/nn_variants.py against the host code of csrc/nn_kernels.cu (132 SMs)"""
+    P = nv.plan
+    # mr_bias_relu_pool_fwd: the row kernel needs a 2x2 window and a power-of-two channel-vector count <= 256
+    assert P("mr_bias_relu_pool_fwd", "bf16", 512, 16, 128, 128, (2, 2), (2, 2), (0, 0)) == {"pool_fwd_rows_kernel<bf16,2,2>"}
+    assert P("mr_bias_relu_pool_fwd", "float", 2, 8, 8, 24, (2, 2), (2, 2), (0, 0)) == {"bias_relu_pool_fwd_kernel<float>"}
+    assert P("mr_bias_relu_pool_fwd", "bf16", 1, 8, 8, 4096, (2, 2), (2, 2), (0, 0)) == {"bias_relu_pool_fwd_kernel<bf16>"}
+    # mr_bias_relu_pool_bwd: tiled / hpair / rows / generic, partials for the fused bias gradient
+    assert P("mr_bias_relu_pool_bwd", "bf16", 512, 16, 128, 128, (2, 2), (2, 2), (0, 0)) == {
+        "pool_bwd_tiled_rows_kernel<bf16,2,2>", "partials_finalize_kernel", "sums_to_float_kernel"}
+    assert "pool_bwd_hpair_rows_kernel<bf16,2>" in P("mr_bias_relu_pool_bwd", "bf16", 512, 8, 64, 256, (2, 2), (2, 1), (0, 1))
+    assert "pool_bwd_hpair_rows_kernel<bf16,2>" in P("mr_bias_relu_pool_bwd", "bf16", 512, 4, 65, 512, (2, 2), (2, 1), (0, 1))
+    assert "pool_bwd_rows_kernel<float,2,2>" in P("mr_bias_relu_pool_bwd", "float", 1, 9, 9, 64, (2, 2), (1, 1), (0, 0))
+    assert "pool_bwd_rows_kernel<float,2,2>" in P("mr_bias_relu_pool_bwd", "float", 1, 5, 8, 64, (2, 2), (2, 2), (0, 0))
+    assert P("mr_bias_relu_pool_bwd", "float", 2, 9, 9, 64, (3, 3), (3, 3), (0, 0), want_dbias=False) == {
+        "bias_relu_pool_bwd_tiled_kernel<float>"}
+    assert P("mr_bias_relu_pool_bwd", "float", 2, 8, 8, 24, (2, 2), (2, 2), (0, 0)) == {
+        "bias_relu_pool_bwd_tiled_kernel<float>", "col_reduce_kernel<float,2>", "partials_finalize_kernel",
+        "sums_to_float_kernel"}                                 # 256 % 6 != 0: the bias gradient is a column sum
+    assert nv.pool_bwd("bf16", 2, 8, 8, 64, (2, 2), (2, 2), (0, 0), scratch=False)[0] == {
+        "bias_relu_pool_bwd_tiled_kernel<bf16>", "sums_to_float_kernel"}       # fp64 atomics: allocation failed only
+    # launch_reduce: partials unless 2C > 4096
+    assert nv.reduce_plan(0, "float", 262144, 256)[1] == "partials"
+    assert nv.reduce_plan(0, "bf16", 4096, 2048)[1] == "partials"
+    assert nv.reduce_plan(0, "bf16", 4096, 2056)[1] == "atomics"
+    assert nv.reduce_plan(2, "float", 10 ** 9, 4)[1] == "partials"
+    # BatchNorm: row kernels iff the channel-vector count divides 256
+    assert P("mr_bn_train_fwd", "bf16", 262144, 256) == {"col_reduce_kernel<bf16,0>", "partials_finalize_kernel",
+                                                          "bn_finalize_kernel<bf16>", "bn_apply_rows_kernel<bf16>"}
+    assert "bn_apply_kernel<float>" in P("mr_bn_train_fwd", "float", 100, 24)
+    assert nv.bn_train_bwd("float", 262144, 24)[2] == "partials" and \
+        "bn_bwd_apply_kernel<float>" in P("mr_bn_train_bwd", "float", 262144, 24)
+    assert nv.bn_train_bwd("bf16", 4096, 2056)[1:] == ("atomics", "atomics")
+    assert nv.bn_bwd_apply_branches("float", 262144, 24) == {"two", "single"}
+    assert nv.bn_bwd_apply_branches("bf16", 262144, 40) == {"differs", "single"}
+    assert nv.bn_bwd_apply_branches("float", 1000, 24) == {"single"}
+    with pytest.raises(nv.Unsupported):
+        nv.bn_apply("float", 10, 6)
+    # small entries
+    assert P("mr_colsum", "float", 500, 38) == {"colsum_scalar_kernel<float>", "sums_to_float_kernel"}
+    assert P("mr_bias_act", "bf16", 10, 38) == {"bias_act_scalar_kernel<bf16>"}
+    assert P("mr_im2col_nhwc", "float", 3, 27) == {"im2col_scalar_kernel<float>"}
+    assert P("mr_im2col_nhwc", "float", 8, 74) == {"im2col_scalar_kernel<float>"}           # Kp % 4 != 0
+    with pytest.raises(nv.Unsupported):
+        nv.col2im("bf16", 3, 32)
+    assert nv.nn_normalise("void (anonymous namespace)::cast_kernel<float, __nv_bfloat16>(float const*, long, "
+                           "__nv_bfloat16*)") == "cast_kernel<float,bf16>"
+    assert nv.nn_normalise("void <unnamed>::pool_bwd_tiled_rows_kernel<__nv_bfloat16, (int)2, (int)2>(<unnamed>::PoolGeo)") \
+        == "pool_bwd_tiled_rows_kernel<bf16,2,2>"
+    assert nv.nn_normalise("<unnamed>::partials_finalize_kernel(const float *, int, int, double *)") == \
+        "partials_finalize_kernel"
