@@ -686,6 +686,33 @@ int mr_image_decode(const void *data, int64_t data_bytes, const int64_t *data_of
                     void *workspace, int64_t workspace_bytes, unsigned char *image_out, int64_t *image_offsets, int *shapes, int *status,
                     void *stream);
 
+/* Lexicon-constrained CTC decoding (Shi, Bai & Yao 2015 §2.3.2; csrc/lexicon.cu; DESIGN §7) of N samples of a CTC head's eval
+ * output: prob [N, C, H, W] class scores with element strides (sN, sC, sH, sW) and mask (nullable: the 1D heads, H = 1) with
+ * strides (mN, mH, mW).  lp[t, h, c] = log(max(mask * prob, tiny)); the score of a word is its 2D-CTC log-likelihood over
+ * input length W (ordinary CTC for H = 1), -inf when it cannot be aligned in W frames.  Word table: n_words words as class ids
+ * word_cls [word_offsets[n_words]] int32 with word_offsets [n_words + 1] int32, each of 1..MR_LEXICON_MAX_WORD classes other
+ * than blank and below C.  ranges [N, 2] int64 (nullable: every sample reads the whole table): sample n's words are
+ * [ranges[n][0], ranges[n][1]).  Its candidates are the words whose Levenshtein distance to its greedy labels
+ * (mr_ctc_greedy_decode) is at most max_edit_distance (-1: every word of the range).  Outputs: labels [N, W] int32 (the
+ * candidate with the largest finite score, the lowest index on a tie, blank-padded; the greedy labels when there is none),
+ * word [N] int32 (-1 for none), score [N] float, candidates [N] int32 (the number scored) and status [N] int32:
+ * MR_LEXICON_OVERFLOW for a range longer than max_words_per_sample, MR_LEXICON_BAD_RANGE for a range outside the table
+ * (both decode nothing and keep the greedy labels), MR_LEXICON_BAD_WORD for a word of the range that breaks the table's rules
+ * (skipped).  workspace >= mr_lexicon_workspace_bytes(N, max_words_per_sample) (0 for N outside 0..65535 or more than 2^33
+ * candidate slots).  MR_ERR_BAD_SHAPE / MR_ERR_NULL_POINTER / MR_ERR_BLANK_RANGE before any CUDA call; MR_ERR_UNSUPPORTED when
+ * W x C log-probabilities do not fit in shared memory.  No allocation and no host synchronisation: the call can be captured
+ * in a CUDA graph and replayed with new probabilities and ranges. */
+#define MR_LEXICON_MAX_WORD 64
+#define MR_LEXICON_OVERFLOW 1
+#define MR_LEXICON_BAD_RANGE 2
+#define MR_LEXICON_BAD_WORD 4
+int64_t mr_lexicon_workspace_bytes(int64_t N, int64_t max_words_per_sample);
+int mr_lexicon_ctc_decode(const float *prob, const float *mask, int N, int C, int H, int W, int64_t sN, int64_t sC, int64_t sH,
+                          int64_t sW, int64_t mN, int64_t mH, int64_t mW, int blank, int unknown, float tiny, const int *word_cls,
+                          const int *word_offsets, int n_words, const long long *ranges, int max_words_per_sample,
+                          int max_edit_distance, void *workspace, int64_t workspace_bytes, int *labels, int *word, float *score,
+                          int *candidates, int *status, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -133,6 +133,9 @@ _SIGS = {
     "mr_rec_measure_workspace_bytes": [c_i64, c_i64, c_i64, c_int],
     "mr_rec_measure": [c_p, c_int, c_p, c_int, c_p, c_int, c_p, c_int, c_int, c_p, c_p, c_int, c_p, c_p, c_int, c_p, c_p, c_i64]
                       + [c_p] * 9,
+    "mr_lexicon_workspace_bytes": [c_i64, c_i64],
+    "mr_lexicon_ctc_decode": [c_p, c_p] + [c_int] * 4 + [c_i64] * 7 + [c_int, c_int, c_f32, c_p, c_p, c_int, c_p, c_int, c_int,
+                                                                     c_p, c_i64] + [c_p] * 6,
 }
 _RESTYPES = {
     "mr_db_contours_workspace_bytes": c_i64,
@@ -142,6 +145,7 @@ _RESTYPES = {
     "mr_db_measure_workspace_bytes": c_i64,
     "mr_rec_lexicon_build_bytes": c_i64,
     "mr_rec_measure_workspace_bytes": c_i64,
+    "mr_lexicon_workspace_bytes": c_i64,
     "mr_db_batch_workspace_bytes": c_i64,
     "mr_text_crop_workspace_bytes": c_i64,
     "mr_jpeg_workspace_bytes": c_i64,
